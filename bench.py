@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """bench.py -- image-pairs/s of the dense-descriptor training hot path (fwd(A) + fwd(B) + loss + backward) at 640x480.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c5] [--two-calls]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c5] [--two-calls] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
 One JSON line on stdout (rank 0).  Workload (default `--config c2`) = BASELINE.json configs[1] ("batch 8 pairs, Resnet34_8s
-D=3, single B200, fused fwd+loss+bwd") per GPU; N GPUs = weak scaling, 8 pairs per GPU, the gradient all-reduce OVERLAPPED
+D=3, single GPU, fused fwd+loss+bwd") per GPU; N GPUs = weak scaling, 8 pairs per GPU, the gradient all-reduce OVERLAPPED
 with the backward (configs[3] at N=8).  `--config c5` (or DDN_BENCH_CONFIG=c5) = BASELINE.json configs[4]: 32 pairs over 8 GPUs
 = 4 pairs per GPU, D=8, 1000 matches + 5000 masked + 5000 background non-matches per pair, hard-negative scaling.  Inputs are
 synthetic (pdc_b200.synthetic, SURVEY.md 8d), weights are the reference's own random init.
@@ -24,6 +24,10 @@ synthetic (pdc_b200.synthetic, SURVEY.md 8d), weights are the reference's own ra
   cpu_baseline     the CPU oracle port of the same step on this box's host cores (bounded sample)
   allreduce_check  (N > 1) the overlapped all-reduce left bit-identical gradients on every rank, equal to the mean of the
                    ranks' local gradients
+
+``--dump-outputs DIR`` writes what the last timed step returned to its caller (see dump_outputs) as DIR/<name>.npy, so that two
+builds can be compared output for output: the inputs and the initial weights are seeded, identical on every run with the same
+arguments.
 
 ``--impl reference`` times the reference's own algorithm on the host CPU (the oracle port, pinned bit-for-bit to the
 executed reference source by tests/test_oracle_ref_cpu.py; the reference itself is Python 2 + needs its dataset stack, so it
@@ -59,11 +63,12 @@ def flops_per_pair(D, H, W):
 
 
 def measured_peaks():
+    """(HBM GB/s, dense bf16 TFLOP/s, source): MEASURED_PEAKS.json if present, else NVIDIA's H100 SXM data sheet (700 W)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 def load_synthetic():
@@ -81,13 +86,14 @@ class ClockSampler(object):
 
     def __init__(self, index):
         self.index, self.samples, self.reasons, self._stop = index, [], set(), threading.Event()
-        self.max_mhz = None
+        self.max_mhz = self.power_limit_w = None
         try:
             import pynvml
             pynvml.nvmlInit()
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
         except Exception:
             self.nv = None
         self.t = threading.Thread(target=self._run, daemon=True)
@@ -122,7 +128,8 @@ class ClockSampler(object):
 
     def summary(self):
         s = sorted(self.samples)
-        return {"sm_mhz": (s[len(s) // 2] if s else None), "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
+        return {"sm_mhz": (s[len(s) // 2] if s else None), "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
+                "reasons": sorted(self.reasons),
                 "samples": len(s)}
 
 
@@ -330,17 +337,32 @@ def gpu_torch_baseline_leg(cfg, H, W, dev):
     return {"workload": "same step as `value` (inputs resident), 3 timed steps after 2 warm-up", "rows": rows}
 
 
-def committed_traffic(kernel_class):
-    """dram bytes per launch of the dominant kernel class from the committed `ncu --set full` capture, if there is one."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(p):
-        try:
-            d = json.load(open(p))
-            if kernel_class in d:
-                return d[kernel_class].get("dram_bytes_per_launch"), d[kernel_class].get("source")
-        except Exception:
-            pass
-    return None, None
+DUMP_SAMPLE = 1 << 20
+
+
+def dump_outputs(out_dir, five, descriptors, flat_gradient, named_params):
+    """The arrays the timed step hands its caller, from its last step: the five loss terms of loss_composer.get_loss (float64),
+    the descriptor images of both forward calls and the whole parameter gradient (float32).  The two descriptor images and the
+    flat gradient are sampled at DUMP_SAMPLE fixed positions each (seeded, the same on every run with the same arguments); the
+    last layer's gradients are stored whole, and every parameter tensor's gradient norm (float64, named_parameters order).
+    ~13 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+
+    def sample(t):
+        flat = t.detach().reshape(-1)
+        idx = np.sort(rng.choice(flat.numel(), size=min(DUMP_SAMPLE, flat.numel()), replace=False))
+        return flat[torch.from_numpy(idx).to(flat.device)].float().cpu().numpy()
+    out = {"loss_terms": np.array([float(t) for t in five], dtype=np.float64),
+           "descriptors_a_sample": sample(descriptors[0]), "descriptors_b_sample": sample(descriptors[1]),
+           "grad_sample": sample(flat_gradient),
+           "grad_norms": np.array([float(p.grad.double().norm()) for _, p in named_params], dtype=np.float64)}
+    for name, p in named_params:
+        if name.endswith(("fc.weight", "fc.bias")):
+            out["grad_" + name.split(".")[-2] + "_" + name.split(".")[-1]] = p.grad.detach().float().cpu().numpy()
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU arm
@@ -388,6 +410,7 @@ def run_ours(args, cfg):
     h2d_bytes = sum(pinned[k].numel() * pinned[k].element_size() for k in keys)
 
     side = [torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)] if args.two_streams else None
+    last = {}                                               # what the latest step returned (--dump-outputs)
 
     def forward_loss_backward(d):
         if args.two_streams:      # EXPERIMENT (timing only: shared BN buffers / pack cache / flat gradient are raced)
@@ -408,6 +431,7 @@ def run_ours(args, cfg):
                                       d["matches_a"], d["matches_b"], d["masked_a"], d["masked_b"],
                                       d["background_a"], d["background_b"], blind, blind)
         five[0].backward()
+        last["five"], last["descriptors"] = five, (ya, yb)
         return five[0]
 
     def step(d):
@@ -453,6 +477,8 @@ def run_ours(args, cfg):
 
     with ClockSampler(local_rank) as clk:
         ms_total, launches, loss, host_ms = timed_steps(False)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["five"], last["descriptors"], dcn.fcn.flat_gradient, list(dcn.fcn.named_parameters()))
     # ---- timed region 1b: the same K steps again with a CUDA-event pair around every convolution / loss kernel on the launching
     # stream (ddn_profile_*): the per-class kernel durations the roofline block is computed from
     if args.profile_run:      # under ncu: warm-up + the timed steps only, so the launch list is exactly `steps` steps
@@ -531,7 +557,7 @@ def run_ours(args, cfg):
         flags = torch.tensor([1.0 if identical else 0.0, -err], device=dev, dtype=torch.float64)
         dist.all_reduce(flags, op=dist.ReduceOp.MIN)
         all_identical, worst_err = bool(flags[0].item() == 1.0), -float(flags[1].item())
-        # the two runs differ by the summation order of the weight-gradient atomics (~1e-6 relative), never by more
+        # the two runs differ by the summation order of the all-reduce and of fp64 sums, never by more than ~1e-6 relative
         allreduce_check = bool(all_identical and worst_err < 1e-4)
         allreduce_detail = {"bit_identical_across_ranks": all_identical, "rel_err_vs_mean_of_local_gradients": worst_err,
                             "overlapped_steps": overlapped_steps, "bytes_per_step": bytes_last}
@@ -551,11 +577,9 @@ def run_ours(args, cfg):
     if dom:
         a = prof[dom]["flops"] / (prof[dom]["ms"] * 1e-3) / 1e12 if prof[dom]["ms"] > 0 else 0.0
         mma_per_mac = {"fp32": 0, "bf16x3": 3, "bf16": 1}[prec_name]
-        traffic, traffic_src = committed_traffic(dom)
         roof = {"bound": "tensor", "kernel": dom, "achieved": a, "peak": tf_peak, "unit": "TFLOP/s", "frac": a / tf_peak,
-                "traffic": traffic, "traffic_source": traffic_src,
                 "issued_tensor_TFLOPs": a * mma_per_mac, "issued_frac": a * mma_per_mac / tf_peak,
-                "peak_source": peak_src + " bf16_tflops_sustained (kernel timed inside a long step)",
+                "peak_source": peak_src + " dense bf16 (kernel timed inside a long step)",
                 "launches": prof[dom]["launches"], "avg_launch_ms": prof[dom]["ms"] / max(1, prof[dom]["launches"]),
                 "all_conv_achieved": (conv_fl / (conv_ms * 1e-3) / 1e12) if conv_ms > 0 else 0.0,
                 "conv_share_of_step": conv_ms / ms_instrumented if ms_instrumented > 0 else None,
@@ -583,7 +607,7 @@ def run_ours(args, cfg):
         "metric": "image-pairs/s (640x480, D=%d) fwd+loss+bwd" % D, "value": value, "unit": "pairs/s",
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_total / args.steps,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": {"fp32": "f32", "bf16x3": "f32 (bf16x3 split on tcgen05, fp32 accumulate)", "bf16": "bf16"}[prec_name],
+        "dtype": {"fp32": "f32", "bf16x3": "f32 (bf16x3 split on the wgmma tensor cores, fp32 accumulate)", "bf16": "bf16"}[prec_name],
         "data": "synthetic",
         "config": {"workload": workload_text(cfg, H, W, ", no optimizer step"),
                    "api": ("DenseCorrespondenceNetwork.forward(A), .forward(B)" if args.two_calls else
@@ -593,8 +617,9 @@ def run_ours(args, cfg):
                    "parallelism": "dp%d" % world, "precision": prec_name,
                    "allreduce": (None if world == 1 else ("overlapped with backward (4 buckets, issued as each residual layer's gradients "
                                                           "complete)" if not args.no_overlap else "after backward")),
-                   "l2": "inputs+activations touched per step (~%.1f GB) are far larger than the 126 MB L2; no explicit flush" %
+                   "l2": "inputs+activations touched per step (~%.1f GB) are far larger than the 50 MB L2; no explicit flush" %
                          (N.lib.ddn_resnet34_8s_workspace_bytes(2 * Bp, H, W, D, 1, prec) / 1e9)},
+        "gpu": torch.cuda.get_device_name(dev),
         "clocks": clk.summary(),
         "e2e": {"value": e2e, "unit": "pairs/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps, "last_loss": last_loss},
@@ -641,6 +666,8 @@ def main():
     ap.add_argument("--no-overlap", action="store_true", help="N > 1: all-reduce after backward instead of overlapped with it")
     ap.add_argument("--l2-pixel-loss", action="store_true",
                     help="configs[4] variant: use_l2_pixel_loss_on_masked_non_matches=True (M_pixel=50)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (see dump_outputs)")
     ap.add_argument("--profile-run", action="store_true",
                     help="short run for ncu: 1 warm-up + --steps timed steps, no e2e / cpu legs (numbers printed are NOT bench values)")
     args = ap.parse_args()
@@ -658,6 +685,8 @@ def main():
     if cfg != CONFIGS[args.config]:
         cfg["name"] = "custom (from %s)" % cfg["name"]
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what this library's timed step computed; the reference arm (--impl reference) has no such step")
         return run_reference_arm(args, cfg)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.gpus != world:

@@ -1,6 +1,6 @@
-/* ddn_b200.h -- C ABI of the B200-native dense-descriptor training path.
+/* ddn_b200.h -- C ABI of the H100-native dense-descriptor training path.
  *
- * One shared library (libddn_b200.so, sm_100a only) exports everything below with C linkage:
+ * One shared library (libddn_b200.so, sm_90a only) exports everything below with C linkage:
  * plain pointers and sizes, no torch / C++ types.  All pointers are DEVICE pointers unless the
  * name ends in _host; `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
  * Every function returns 0 on success, a negative DDN_E* code on a contract violation and a
@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define DDN_ABI_VERSION 2
+#define DDN_ABI_VERSION 3
 
 enum {
   DDN_OK = 0,
@@ -34,8 +34,8 @@ enum {
 /* Arithmetic used by the convolution contractions. */
 enum {
   DDN_PRECISION_FP32_SIMT = 0, /* fp32 FFMA on CUDA cores (bit-for-bit class of the fp32 oracle)        */
-  DDN_PRECISION_BF16X3 = 1,    /* tcgen05, operands split hi+lo bf16, 3 MMAs, fp32 accumulate in TMEM   */
-  DDN_PRECISION_BF16 = 2       /* tcgen05, single bf16 pass ("fast mode"; fails the 1e-3 descriptor gate) */
+  DDN_PRECISION_BF16X3 = 1,    /* wgmma, operands split hi+lo bf16, 3 MMAs, fp32 accumulate            */
+  DDN_PRECISION_BF16 = 2       /* wgmma, single bf16 pass ("fast mode"; fails the 1e-3 descriptor gate)   */
 };
 
 int ddn_abi_version(void);
@@ -185,14 +185,16 @@ int ddn_contrastive_terms_backward(const float* pred_a, const float* pred_b,
  * (`low_nhwc_out` of ddn_resnet34_8s_forward), index tensors still address the H x W image.  Each descriptor is blended from
  * its 4 low-resolution cells (identical fp32 arithmetic to ddn_upsample_bilinear_forward), so sums / counts equal those of
  * the entry points above on the upsampled image; the backward scatters into d(low) [B, h*w, D] (caller zero-fills), which
- * ddn_resnet34_8s_backward takes as `dlow_nhwc` -- the full-resolution image and its gradient are never touched. */
+ * ddn_resnet34_8s_backward takes as `dlow_nhwc` -- the full-resolution image and its gradient are never touched.  The scatter
+ * accumulates in fp64 so that its result does not depend on the order in which pairs arrive: `scratch` = 2 * B*h*w*D doubles
+ * (any contents; 16-byte aligned) holds that accumulator, which is then added to dlow_a / dlow_b. */
 int ddn_contrastive_terms_forward_lowres(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
                                          const ddn_loss_term* terms_host, int n_terms,
                                          double* sums, int64_t* counts, void* stream);
 int ddn_contrastive_terms_backward_lowres(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
                                           const ddn_loss_term* terms_host, int n_terms,
                                           const float* coef, const float* upstream,
-                                          float* dlow_a, float* dlow_b, void* stream);
+                                          float* dlow_a, float* dlow_b, double* scratch, void* stream);
 
 /* loss_composer.get_within_scene_loss (dense_correspondence/loss_functions/loss_composer.py:70-143)
  * evaluated on the device from the sums/counts of terms ordered {match, masked, background[, blind]}:

@@ -1,9 +1,9 @@
 """Builds oracle/_ref/: the reference's OWN loss / composer / correspondence-finder sources, made importable.
 
-TEST INFRASTRUCTURE (build container only -- needs /root/reference).  Nothing is copied into the repository:
+TEST INFRASTRUCTURE (needs a checkout of the reference, PDC_REFERENCE_ROOT).  Nothing is copied into the repository:
 the reference files are read where they lie, a short list of documented, LINE-ANCHORED Python-2 -> Python-3
 patches is applied in memory, and the result is written to the git-ignored directory oracle/_ref/ (it travels to
-the GPU box with the snapshot like a built .so, but never enters history).  Every patch names the reference line it
+a test machine like a built .so, but never enters history).  Every patch names the reference line it
 touches and must match that line's text exactly, so a different reference revision fails loudly instead of being
 silently mis-patched.  What is executed afterwards IS the reference's code:
 
@@ -27,7 +27,8 @@ import re
 import sys
 import textwrap
 
-REF_ROOT = "/root/reference"
+# a checkout of RobotLocomotion/pytorch-dense-correspondence (with its external/ submodules)
+REF_ROOT = os.environ.get("PDC_REFERENCE_ROOT") or None
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "_ref")
 
@@ -48,7 +49,7 @@ PATCHES = {
         (50, 'print "applying MULTI_OBJECT loss"', 'print("applying MULTI_OBJECT loss")', "print statement"),
         (59, 'print "applying SYNTHETIC_MULTI_OBJECT loss"', 'print("applying SYNTHETIC_MULTI_OBJECT loss")', "print statement"),
         (215, "Variable(torch.FloatTensor([0]).cuda())", "Variable(torch.FloatTensor([0]))",
-         "the oracle runs on the CPU (no GPU in the build container); value unchanged"),
+         "the oracle runs on the CPU; value unchanged"),
     ],
     "dense_correspondence/correspondence_tools/correspondence_finder.py": [
         (322, 'print "warning, empty mask b"', 'print("warning, empty mask b")', "print statement"),
@@ -74,7 +75,7 @@ CUTS = {
 
 
 def reference_available():
-    return all(os.path.isfile(os.path.join(REF_ROOT, p)) for p in PATCHES)
+    return REF_ROOT is not None and all(os.path.isfile(os.path.join(REF_ROOT, p)) for p in PATCHES)
 
 
 def _lines(rel):
@@ -110,7 +111,7 @@ def _write(rel, text):
 
 def build(verbose=False):
     if not reference_available():
-        raise RuntimeError("needs %s (build container only)" % REF_ROOT)
+        raise RuntimeError("set PDC_REFERENCE_ROOT to a checkout of the reference (now %r)" % REF_ROOT)
     log = []
     for rel in PATCHES:
         _write(rel, "# GENERATED by oracle/build_ref.py from %s/%s -- do not commit\n" % (REF_ROOT, rel) + _patched(rel, log))

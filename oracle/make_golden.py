@@ -1,6 +1,6 @@
 """Pins the oracle against the real reference and writes tests/golden/*.npz.
 
-Run in the BUILD CONTAINER only (needs /root/reference):   python oracle/make_golden.py
+Needs a checkout of the reference (PDC_REFERENCE_ROOT=<dir>):   python oracle/make_golden.py [reference_checks]
 
 For every backbone case the REAL reference module (loaded unmodified by oracle/ref_loader.py)
 and the oracle restatement are run on the same seeded weights and inputs and must agree
@@ -137,10 +137,94 @@ def train_step_case(name, D, B, H, W, Nm, Nn, seed):
     print("wrote", name, "five", out["five"])
 
 
+def _same(a, b, what):
+    assert a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a, b), what
+
+
+def reference_checks():
+    """tests/golden/reference_checks.npz: the executed reference's results on every case of oracle/ref_cases.py (and the
+    backbone modules on a small input), each required here to equal the restatement's bit-for-bit."""
+    from oracle import ref_cases as RC
+    ref = build_ref.load()
+    out = {}
+    # loss: every method, every composer branch
+    r = RC.every_loss_method(ref.pcl.PixelwiseContrastiveLoss)
+    o = RC.every_loss_method(LO.TorchPixelwiseContrastiveLoss)
+    assert sorted(r) == sorted(o)
+    for k in r:
+        _same(o[k], r[k], k)
+        out["method/" + k] = r[k]
+    r = RC.composer_branches(ref.pcl.PixelwiseContrastiveLoss, ref.composer.get_loss, ref.dataset.SpartanDataset.empty_tensor)
+    o = RC.composer_branches(LO.TorchPixelwiseContrastiveLoss, LO.get_loss, LO.empty_tensor)
+    assert sorted(r) == sorted(o)
+    for k in r:
+        _same(o[k], r[k], k)
+        out["composer/" + k] = r[k]
+    for k in dir(ref.dataset.SpartanDatasetDataType):
+        if k.isupper():
+            out["datatype/" + k] = np.array(getattr(ref.dataset.SpartanDatasetDataType, k))
+    # the non-match sampler: create_non_correspondences draws torch.rand(n) (mask branch) or torch.rand(2, n) (no mask), then two
+    # more draws for the no-op perturbation -- it is given the uniforms the restatement takes as arguments
+    H, W, k, ma, ru, rv, masks = RC.sampler_inputs()
+    uv_a = (ma % W, ma // W)
+    uv_b = ((ma % W).float(), (ma // W).float())
+    n = len(ma) * k
+    real_rand = ref.finder.torch.rand
+    for i, m in enumerate(masks):
+        calls = []
+
+        def fake_rand(*shape):
+            calls.append(shape)
+            if len(calls) == 1:
+                return ru.clone() if shape == (n,) else torch.stack((ru, rv)).clone()
+            return torch.zeros(*shape)
+        ref.finder.torch.rand = fake_rand
+        try:
+            uv_b_non = ref.finder.create_non_correspondences(uv_b, (H, W), num_non_matches_per_match=k, img_b_mask=m)
+        finally:
+            ref.finder.torch.rand = real_rand
+        SD = ref.dataset.SpartanDataset
+        uv_a_long, uv_b_long = SD.create_non_matches(None, uv_a, uv_b_non, k)
+        na_r = SD.flatten_uv_tensor(uv_a_long, W).squeeze(1); nb_r = SD.flatten_uv_tensor(uv_b_long, W).squeeze(1)
+        na_o, nb_o = LO.create_non_correspondences_flat(ma, (H, W), k, m, ru, rv)
+        assert torch.equal(na_o, na_r) and torch.equal(nb_o, nb_r)
+        out["sampler/%d/a" % i], out["sampler/%d/b" % i] = na_r.numpy(), nb_r.numpy()
+    # the reprojection match finder: it first draws (and discards) rand(2, n) for unmasked candidates, then rand(n)
+    da, pa, db, pb, mask, ru, K, n = RC.reprojection_scene()
+    ref.finder.torch.rand = lambda *s: ru.clone() if s == (n,) else torch.zeros(*s)
+    try:
+        uv_a_r, uv_b_r = ref.finder.batch_find_pixel_correspondences(da, pa, db, pb, num_attempts=n, img_a_mask=mask, K=K)
+    finally:
+        ref.finder.torch.rand = real_rand
+    for i, t in enumerate(uv_a_r + uv_b_r):
+        out["reprojection/%d" % i] = t.numpy()
+    # the backbone modules, train and eval, and the dilation bookkeeping the modern torchvision API gets differently
+    D = 8
+    oracle = seeded_oracle(D=D, seed=0)
+    refnet = ref_loader.reference_resnet34_8s(D, oracle.state_dict())
+    out["backbone/keys"] = np.array(list(refnet.state_dict().keys()))
+    x = torch.randn(1, 3, 40, 56, generator=torch.Generator().manual_seed(2))
+    for mode in ("train", "eval"):
+        getattr(refnet, mode)(); getattr(oracle, mode)()
+        with torch.no_grad():
+            y = refnet(x)
+            bit_equal(y, oracle(x), "backbone " + mode)
+        out["backbone/" + mode] = y.numpy()
+    r = refnet.resnet34_8s
+    out["backbone/geometry"] = np.array([r.layer3[0].conv1.dilation[0], r.layer3[0].conv1.padding[0], r.layer4[0].conv1.dilation[0],
+                                         r.layer4[0].downsample[0].stride[0], r.layer2[0].conv1.stride[0],
+                                         r.layer2[0].downsample[0].stride[0]])
+    np.savez_compressed(os.path.join(GOLD, "reference_checks.npz"), **out)
+    print("wrote reference_checks", len(out), "arrays")
+
+
 if __name__ == "__main__":
-    assert ref_loader.reference_available() and build_ref.reference_available(), "needs /root/reference"
+    assert ref_loader.reference_available() and build_ref.reference_available(), "set PDC_REFERENCE_ROOT to a checkout of the reference"
     build_ref.build()
     os.makedirs(GOLD, exist_ok=True)
+    if sys.argv[1:] == ["reference_checks"]:      # only the cross-check file (the other goldens stay as they are)
+        reference_checks()
+        sys.exit(0)
     backbone_case("backbone_small_d3", D=3, B=2, H=64, W=96, seed_data=11)
     backbone_case("backbone_small_d16", D=16, B=1, H=48, W=64, seed_data=12)
     backbone_case("backbone_full_d3", D=3, B=1, H=480, W=640, seed_data=13)
@@ -151,3 +235,4 @@ if __name__ == "__main__":
     loss_case("loss_noscale_d16", 16, 48, 64, 64, 2, 1, 5, {"scale_by_hard_negatives": False, "M_masked": 1.5,
                                                              "M_background": 1.2}, 23)
     train_step_case("train_step_small_d3", D=3, B=2, H=64, W=96, Nm=40, Nn=120, seed=31)
+    reference_checks()

@@ -1,8 +1,7 @@
-"""Loads the REAL reference backbone from /root/reference by file path -- build container only.
+"""Loads the REAL reference backbone by file path from the reference checkout (PDC_REFERENCE_ROOT).
 
-TEST INFRASTRUCTURE.  /root/reference does not exist on the GPU box, so nothing that runs there
-may call this; it is used by oracle/make_golden.py (which writes tests/golden/) and by the
-``not gpu`` test that re-checks oracle == reference when the tree is present.
+TEST INFRASTRUCTURE.  The tests must not need the reference checkout, so nothing they run
+may call this; oracle/make_golden.py uses it to write tests/golden/.
 
 Recipe (SURVEY.md appendix D): exec the vendored torchvision-fork resnet.py and
 pytorch_segmentation_detection/models/resnet_dilated.py unmodified, with (1) a shim module bound
@@ -15,14 +14,14 @@ import os
 import sys
 import types
 
-REF_ROOT = "/root/reference"
-_PSD = os.path.join(REF_ROOT, "external", "pytorch-segmentation-detection")
-TV_RESNET = os.path.join(_PSD, "vision", "torchvision", "models", "resnet.py")
-RESNET_DILATED = os.path.join(_PSD, "pytorch_segmentation_detection", "models", "resnet_dilated.py")
+from oracle.build_ref import REF_ROOT
+_PSD = os.path.join(REF_ROOT, "external", "pytorch-segmentation-detection") if REF_ROOT else None
+TV_RESNET = os.path.join(_PSD, "vision", "torchvision", "models", "resnet.py") if _PSD else None
+RESNET_DILATED = os.path.join(_PSD, "pytorch_segmentation_detection", "models", "resnet_dilated.py") if _PSD else None
 
 
 def reference_available():
-    return os.path.isfile(TV_RESNET) and os.path.isfile(RESNET_DILATED)
+    return _PSD is not None and os.path.isfile(TV_RESNET) and os.path.isfile(RESNET_DILATED)
 
 
 def _load(name, path):

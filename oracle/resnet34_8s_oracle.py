@@ -22,7 +22,7 @@ what is restated here is the reference's *wiring* of those ops:
                                       upsample_bilinear == align_corners=True)
 
 Parity pin: ``oracle/make_golden.py`` imports the real reference modules from
-/root/reference (in the build container), loads this oracle's seeded state_dict
+the reference checkout (PDC_REFERENCE_ROOT), loads this oracle's seeded state_dict
 into them and checks bit-equality of the outputs before writing tests/golden/.
 The reference holds no golden vectors / known-answer tests of its own for this
 path (SURVEY.md section 8c), so "the reference executed on seeded inputs" is the

@@ -1,4 +1,4 @@
-"""pytorch-dense-correspondence_b200 -- the B200-native (sm_100a) implementation of the dense-descriptor training
+"""pytorch-dense-correspondence_b200 -- the H100-native (sm_90a) implementation of the dense-descriptor training
 hot path of RobotLocomotion/pytorch-dense-correspondence: Resnet34_8s forward/backward and the pixelwise
 contrastive loss, behind the reference's own Python API.  Import as ``pdc_b200`` (see pdc_b200.py at the repo
 root; the directory name itself is not a valid Python identifier).

@@ -59,7 +59,7 @@ _SIGNATURES = {
     "ddn_resnet34_8s_backward": (i32, [vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, i32, GRAD_BUCKET_FN, vp, vp]),
     "ddn_contrastive_terms_forward_lowres": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp, vp]),
     "ddn_contrastive_terms_backward_lowres": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32,
-                                                    vp, vp, vp, vp, vp]),
+                                                    vp, vp, vp, vp, vp, vp]),
     "ddn_resnet34_8s_grad_buckets": (i32, [i32, ctypes.POINTER(i64), i32]),
     "ddn_contrastive_terms_forward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp, vp]),
     "ddn_contrastive_terms_backward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32,
@@ -91,7 +91,7 @@ EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
 def _load():
     if not os.path.exists(LIB_PATH):
-        # fresh checkout: compile the library in-tree (nvcc cross-compiles sm_100a without a GPU).  Still no fallback: if
+        # fresh checkout: compile the library in-tree (nvcc cross-compiles sm_90a without a GPU).  Still no fallback: if
         # nvcc is not there either, importing the package fails.
         try:
             import importlib.util
@@ -108,7 +108,7 @@ def _load():
         fn = getattr(lib, name)      # AttributeError here == header/library mismatch: fail loudly
         fn.restype = res
         fn.argtypes = args
-    if lib.ddn_abi_version() != 2:
+    if lib.ddn_abi_version() != 3:
         raise ImportError("libddn_b200.so ABI version mismatch")
     return lib
 

@@ -1,4 +1,4 @@
-"""Builds libddn_b200.so IN-TREE with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libddn_b200.so IN-TREE with nvcc for sm_90a (cross-compiles without a GPU).
 
     python pytorch-dense-correspondence_b200/build.py [--force] [--verbose]
 """
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libddn_b200.so")
 SOURCES = ["engine.cu", "loss.cu", "loss_lowres.cu", "conv_simt.cu", "bn.cu", "head.cu", "conv_tc.cu", "optim.cu", "match.cu", "sampling.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "-cudart", "static"]
 
 
@@ -41,7 +41,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if procs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB, "-cudart", "static"] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB, "-cudart", "static"] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         subprocess.check_call(cmd)
     return LIB
 

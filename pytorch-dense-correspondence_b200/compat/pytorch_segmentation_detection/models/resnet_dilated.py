@@ -1,4 +1,4 @@
-"""Shim for pytorch_segmentation_detection/models/resnet_dilated.py -> the B200 implementation (Resnet34_8s only)."""
+"""Shim for pytorch_segmentation_detection/models/resnet_dilated.py -> this project's implementation (Resnet34_8s only)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import _load  # noqa: F401

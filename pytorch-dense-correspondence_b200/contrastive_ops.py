@@ -203,8 +203,10 @@ class _WithinSceneLowres(torch.autograd.Function):
         da = torch.zeros_like(low_a)
         db = torch.zeros_like(low_b)
         up = dloss.to(torch.float32).contiguous()
+        scratch = torch.empty(2 * low_a.numel(), dtype=torch.float64, device=low_a.device)    # the fp64 scatter accumulator
         N.check(N.lib.ddn_contrastive_terms_backward_lowres(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, ctx.arr, len(ctx.arr),
-                                                            N.ptr(coef), N.ptr(up), N.ptr(da), N.ptr(db), N.stream_ptr()))
+                                                            N.ptr(coef), N.ptr(up), N.ptr(da), N.ptr(db), N.ptr(scratch),
+                                                            N.stream_ptr()))
         return da, db, None, None, None
 
 

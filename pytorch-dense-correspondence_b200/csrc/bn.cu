@@ -6,7 +6,7 @@
 // training = batch mean and BIASED variance over (N,H,W), eps inside the sqrt, running statistics updated
 // with momentum and the UNBIASED variance; eval = running statistics.
 //
-// Byte diet of round 2 (tensor-core modes): activations exist ONLY as bf16 hi/lo operand planes (x ~= hi + lo, 16
+// Byte diet (tensor-core modes): activations exist ONLY as bf16 hi/lo operand planes (x ~= hi + lo, 16
 // mantissa bits -- what every conv reads anyway); the residual add reads the planes, the ReLU mask of a BatchNorm without
 // residual is recomputed from its own input, and column statistics are finalized by the last CTA of the kernel that
 // produced them (bn_stats.cuh) instead of by a second launch.  G > 1: per-group batch statistics (pair-batched step).
@@ -405,7 +405,7 @@ static int check_c(int C, int G, int64_t M) {
 }
 // Grid of a grid-stride kernel = exactly the CTAs that are resident at once (SMs x occupancy): a larger grid runs a second,
 // partial wave at low occupancy AFTER the first one has finished its (already complete-looking) share -- with 40 registers
-// per thread only 6 CTAs of 256 threads fit an SM, and the 8-per-SM grid of round 1 cost these kernels ~1.5x.
+// per thread only 6 CTAs of 256 threads fit an SM, and an 8-per-SM grid costs these kernels ~1.5x.
 template <typename K>
 static int resident_blocks(K kernel, size_t smem) {
   int per_sm = 0;

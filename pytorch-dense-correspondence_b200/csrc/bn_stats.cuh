@@ -4,7 +4,7 @@
 // `red.global.add` into ONE small accumulator [G][2][C]; the CTAs then take a ticket, and the last one to arrive turns
 // the sums into BatchNorm statistics (forward: mean / 1/sqrt(var+eps) / running statistics; backward: dgamma, dbeta and
 // the per-group sums the dx pass needs), zeroes the accumulator and resets the ticket for the next user.  This replaces
-// the per-tile partial-sum buffers + the 288 `bn_*_finalize` launches per step of round 1.
+// per-tile partial-sum buffers and a separate `bn_*_finalize` launch per BatchNorm.
 //
 // G = number of BatchNorm groups in the batch: images [g*B/G, (g+1)*B/G) share one set of batch statistics.  G = 1 is
 // nn.BatchNorm2d over the whole call; G = 2 is the pair-batched step (image A batch and image B batch of

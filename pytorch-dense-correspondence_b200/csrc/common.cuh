@@ -1,4 +1,4 @@
-// Shared helpers for libddn_b200 (sm_100a only).
+// Shared helpers for libddn_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -9,8 +9,8 @@
 
 #include "../../include/ddn_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libddn_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libddn_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace ddn {
@@ -45,7 +45,7 @@ void set_error(const char* fmt, ...);
 // attribute and starts with pdl_prologue(): `launch_dependents` lets the NEXT kernel's CTAs become resident as soon as an
 // SM has room for them (they park in `griddepcontrol.wait`, issuing nothing), and `wait` returns once the PREVIOUS kernel
 // has completed and its memory is visible.  A step is ~230 dependent launches; this removes the drain + launch gap between
-// them (and, in the persistent tcgen05 kernels, overlaps barrier init / TMEM allocation with the predecessor's tail).
+// them (and, in the persistent tensor-core kernels, overlaps barrier initialisation with the predecessor's tail).
 // Rule: nothing written by an earlier kernel may be read before pdl_wait(), and EVERY thread of every kernel executes it
 // (a kernel that skipped it could finish before its predecessor and break the chain for its successor).
 // DDN_PDL=0 launches without the attribute (the instructions are then no-ops).

@@ -8,7 +8,7 @@
 //
 // These kernels are the exact-fp32 class of the oracle (cuDNN/MKLDNN fp32 in the reference:
 // nn.Conv2d at PSD/vision/torchvision/models/resnet.py:36,136,210); they also carry the convs the
-// tcgen05 path does not cover (7x7/2 stem with Cin=3, the two stride-2 convs of layer2).
+// tensor-core path does not cover (7x7/2 stem with Cin=3, the two stride-2 convs of layer2).
 #include "conv.cuh"
 
 namespace ddn {

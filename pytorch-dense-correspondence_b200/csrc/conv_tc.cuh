@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM convolution interface -- see conv_tc.cu.
+// wgmma (Hopper tensor core) implicit-GEMM convolution interface -- see conv_tc.cu.
 #pragma once
 #include "common.cuh"
 #include "bn_stats.cuh"
@@ -44,13 +44,13 @@ int tc_dgrad_strided(const float* dy_f32, TcPlanes up, const float* w_oihw, cons
                      int N, int H, int W, int Cin, int Cout, int k, int precision, void* wws, size_t wws_bytes, cudaStream_t st,
                      const TcBwdStats* bst = nullptr);
 // dw != nullptr: immediate (dwp = scratch, zero-filled and converted here); dw == nullptr: accumulate into the caller's pre-zeroed
-// dwp [taps][Cout][Cin] and convert later with tc_unpack_wgrads (one launch for a whole gradient bucket)
+// fp64 dwp [taps][Cout][Cin] and convert later with tc_unpack_wgrads (one launch for a whole gradient bucket)
 int tc_wgrad_planes(TcPlanes x, TcPlanes dy, float* dw, int N, int H, int W, int Cin, int Cout, int k, int stride, int dil,
-                    int precision, float* dwp, cudaStream_t st);
+                    int precision, double* dwp, cudaStream_t st);
 struct TcUnpackEntry { int64_t src_off, dst_off; int Cout, Cin, taps, kind; };   // kind 1 = stem [64][192] -> [64][3][7][7]
 constexpr int TC_UNPACK_MAX = 40;
 struct TcUnpackTable { TcUnpackEntry e[TC_UNPACK_MAX]; int n; };
-int tc_unpack_wgrads(const TcUnpackEntry* entries, int n, const float* dwp_base, float* grads_base, cudaStream_t st);
+int tc_unpack_wgrads(const TcUnpackEntry* entries, int n, const double* dwp_base, float* grads_base, cudaStream_t st);
 // device-validated cache of every conv's packed weights (see conv_tc.cu "weight-pack cache")
 struct TcPackEntry { int64_t w_off, dst_off; int Cout, Cin, k, dgrad, kind; };   // kind 1 = stem patch-GEMM layout [64][192]
 constexpr int TC_PACK_MAX = 80;
@@ -62,13 +62,13 @@ int tc_stem_patches(const float* x_nchw, __nv_bfloat16* hi, __nv_bfloat16* lo, i
 int tc_stem_pack_weights(const float* w_conv1, __nv_bfloat16* hi, __nv_bfloat16* lo, int precision, cudaStream_t st);   // [64][192]
 int tc_stem_forward(TcPlanes patches, const float* w_conv1, const TcPlanes* w_packed, float* raw, const BnFwdFinal* stats, int N, int H1,
                     int W1, int precision, void* wws, size_t wws_bytes, cudaStream_t st);
-int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1, int W1, int precision, float* scratch, cudaStream_t st);
+int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1, int W1, int precision, double* scratch, cudaStream_t st);
 
 // fp32-tensor wrappers (single-operator C ABI)
 int tc_conv_forward(const float* x_nhwc, const float* w_oihw, float* y_nhwc, int N, int H, int W, int Cin, int Cout,
                     int k, int stride, int pad, int dil, int precision, void* ws, size_t ws_bytes, cudaStream_t st);
 int tc_conv_backward(const float* x_nhwc, const float* w_oihw, const float* dy_nhwc, float* dx_nhwc, const float* dx_addend,
                      float* dw_oihw, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil, int precision,
-                     void* ws, size_t ws_bytes, float* dwp_scratch, cudaStream_t st);
+                     void* ws, size_t ws_bytes, double* dwp_scratch, cudaStream_t st);
 
 }  // namespace ddn

@@ -30,14 +30,13 @@ bool pdl_enabled() {
   return v != 0;
 }
 
-// SMs left free by the persistent tcgen05 kernels (one CTA per SM, no room for a second): while a data-parallel host has a gradient
+// SMs left free by the persistent tensor-core kernels (one CTA per SM, no room for a second): while a data-parallel host has a gradient
 // all-reduce in flight, NCCL's CTAs need somewhere to run -- without the reservation they take SMs between two of our launches and
 // the next persistent kernel runs a whole extra wave for the CTAs that found no SM.  Set by ddn_set_reserved_sms (DDN_RESERVED_SMS).
 static std::atomic<int> g_reserved_sms{-1};
 // ... and the same for a WINDOW only: from the first gradient bucket a backward hands to its host (whose all-reduce then runs
-// concurrently) to the end of that backward (DDN_OVERLAP_RESERVED_SMS = n; the host then caps NCCL at n CTAs).  Measured on
-// 2 x B200 in one call (profiles/r2_reserved_sms_ab.md): n = 0 538, n = 4 545, n = 8 537, n = 16 528 pairs/s -- inside the +-1 %
-// run-to-run noise, so the default is 0 (no reservation, NCCL's own CTA count).
+// concurrently) to the end of that backward (DDN_OVERLAP_RESERVED_SMS = n; the host then caps NCCL at n CTAs).  Default 0
+// (no reservation, NCCL's own CTA count); the effect has not been measured on H100.
 static std::atomic<int> g_window_reserved{0};
 static int overlap_window_sms() {
   static int v = -1;
@@ -57,7 +56,7 @@ int num_sms() {
   if (n == 0) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;                 // H100 SXM
   }
   return n;
 }
@@ -195,8 +194,9 @@ struct Plan {
   std::vector<BlockBufs> blk;
   size_t low, dlow;
   size_t wpack, wpack2, dwp, scratch[4];
+  size_t fc_part;                     // FC_PART_SLOTS x (D*512 + D) floats: per-block partial sums of the fc gradient
   size_t acc, sums;                   // BatchNorm accumulator (bn_stats.cuh) and the backward's per-group sums
-  size_t dwp_all;                     // [n_params + 64*192] floats: every conv's [taps][Cout][Cin] gradient accumulator (tensor-core modes)
+  size_t dwp_all;                     // [n_params + 64*192] doubles: every conv's [taps][Cout][Cin] gradient accumulator (tensor-core modes)
   size_t scratch_elems;
   size_t total;
 };
@@ -209,7 +209,7 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
   DDN_CHECK_ARG(precision >= DDN_PRECISION_FP32_SIMT && precision <= DDN_PRECISION_BF16, "unknown precision %d", precision);
   DDN_CHECK_ARG(mode >= DDN_MODE_INFER && mode <= DDN_MODE_EVAL_SAVE, "unknown mode %d", mode);
   if (precision != DDN_PRECISION_FP32_SIMT && !tc_available()) {
-    set_error("precision %d needs the tcgen05 conv path, which this build does not contain", precision);
+    set_error("precision %d needs the tensor-core conv path, which this build does not contain", precision);
     return DDN_EUNSUPPORTED;
   }
   const NetSpec& s = get_spec(D);
@@ -269,7 +269,8 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
   for (int i = 0; i < 4; ++i) p->scratch[i] = f32((int64_t)max_act);
   p->grad_p = planes(max_act);
   p->wws = alloc(p->tc ? tc_weight_ws_bytes() : 0);
-  p->dwp_all = (p->tc && mode != DDN_MODE_INFER) ? f32(s.n_params + 64 * 192) : 0;
+  p->dwp_all = (p->tc && mode != DDN_MODE_INFER) ? alloc(sizeof(double) * (size_t)(s.n_params + 64 * 192)) : 0;
+  p->fc_part = mode != DDN_MODE_INFER ? f32((int64_t)FC_PART_SLOTS * (D * 512 + D)) : 0;
   p->total = cur;
   return 0;
 }
@@ -278,6 +279,7 @@ struct Ctx {
   const NetSpec* s; const Plan* p; char* ws; const float* params; float* buffers; float* grads;
   cudaStream_t st; float momentum, eps; int mode; int G;
   float* f(size_t off) const { return reinterpret_cast<float*>(ws + off); }
+  double* d(size_t off) const { return reinterpret_cast<double*>(ws + off); }
   __nv_bfloat16* h(size_t off) const { return reinterpret_cast<__nv_bfloat16*>(ws + off); }
   TcPlanes planes(const PlaneBufs& b) const { return TcPlanes{h(b.hi), h(b.lo)}; }
   float* mean(size_t stats) const { return f(stats); }
@@ -513,7 +515,7 @@ static int conv_backward(const Ctx& c, const ConvSpec& cs, const float* in, cons
   const double fl = 2.0 * N * Hout * Wout * (double)cs.cout * cs.k * cs.k * cs.cin;
   if (conv_on_tc(c, cs, Hin, Win)) {
     DDN_TRY(tc_wgrad_planes(c.planes(in_p), c.planes(p.grad_p), nullptr, N, Hin, Win, cs.cin, cs.cout, cs.k, cs.stride, cs.dil,
-                            p.precision, c.f(p.dwp_all) + cs.w_off, c.st));
+                            p.precision, c.d(p.dwp_all) + cs.w_off, c.st));
     if (dx) {
       TcPlanes wpk_s; const TcPlanes* wpk = cached_pack(c, cs, 1, &wpk_s);
       if (cs.stride == 2)   // zero-insert the fp32 dY into the (now free) gradient planes, then an ordinary stride-1 dgrad
@@ -597,7 +599,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   const bool want_lo = p.precision == DDN_PRECISION_BF16X3;
   float* S[4] = {c.f(p.scratch[0]), c.f(p.scratch[1]), c.f(p.scratch[2]), c.f(p.scratch[3])};
   DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(512), c.st));
-  if (p.tc) DDN_CUDA(cudaMemsetAsync(c.f(p.dwp_all), 0, sizeof(float) * (size_t)(s.n_params + 64 * 192), c.st));
+  if (p.tc) DDN_CUDA(cudaMemsetAsync(c.d(p.dwp_all), 0, sizeof(double) * (size_t)(s.n_params + 64 * 192), c.st));
   const BlockBufs& last = p.blk.back();
   // d(low) = upsample^T(dy) [+ the gradient the fused loss scattered straight into the low-resolution map]
   if (dy) DDN_TRY(launch_upsample_bwd(dy, c.f(p.dlow), B * p.D, h8, w8, p.H, p.W, c.st));
@@ -605,7 +607,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   int cur = 0;   // index of the scratch buffer holding d(block output)
   DDN_TRY(launch_fc_backward(c.f(p.dlow), p.tc ? nullptr : c.f(last.out), p.tc ? c.h(last.out_p.hi) : nullptr,
                              (p.tc && want_lo) ? c.h(last.out_p.lo) : nullptr, c.params + s.fc_w, S[cur], c.grads + s.fc_w,
-                             c.grads + s.fc_b, (int64_t)h8 * w8, B, 512, p.D, c.st));
+                             c.grads + s.fc_b, c.f(p.fc_part), (int64_t)h8 * w8, B, 512, p.D, c.st));
   std::vector<TcUnpackEntry> pending;      // tensor-core weight gradients waiting in dwp_all for the bucket's conversion
   auto defer = [&](const ConvSpec& cs, int Hin, int Win) {
     if (!conv_on_tc(c, cs, Hin, Win)) return;
@@ -616,7 +618,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   int bucket_id = 0;
   struct WindowGuard { ~WindowGuard() { g_window_reserved.store(0, std::memory_order_relaxed); } } window_guard;
   auto close_bucket = [&](int64_t begin) -> int {
-    if (!pending.empty()) DDN_TRY(tc_unpack_wgrads(pending.data(), (int)pending.size(), c.f(p.dwp_all), c.grads, c.st));
+    if (!pending.empty()) DDN_TRY(tc_unpack_wgrads(pending.data(), (int)pending.size(), c.d(p.dwp_all), c.grads, c.st));
     pending.clear();
     if (on_bucket) {
       on_bucket(user, bucket_id, begin, bucket_end - begin);
@@ -685,7 +687,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   if (p.tc) {
     ks.dx_hi = c.h(p.grad_p.hi); ks.dx_lo = want_lo ? c.h(p.grad_p.lo) : nullptr;
     DDN_TRY(launch_bn_backward(ks, c.st));
-    DDN_TRY(tc_stem_wgrad(c.planes(p.patch_p), c.planes(p.grad_p), nullptr, B, p.H1, p.W1, p.precision, c.f(p.dwp_all) + s.n_params, c.st));
+    DDN_TRY(tc_stem_wgrad(c.planes(p.patch_p), c.planes(p.grad_p), nullptr, B, p.H1, p.W1, p.precision, c.d(p.dwp_all) + s.n_params, c.st));
     TcUnpackEntry e; e.src_off = s.n_params; e.dst_off = s.stem.w_off; e.Cout = 64; e.Cin = 3; e.taps = 49; e.kind = 1;
     pending.push_back(e);
   } else {
@@ -848,7 +850,7 @@ extern "C" int ddn_conv2d_forward(const float* x, const float* w, float* y, int 
   size_t wb = align_up(sizeof(float) * (size_t)k * k * Cin * Cout, 256);
   int Ho = conv_out(H, k, stride, pad, dil), Wo = conv_out(W, k, stride, pad, dil);
   if (precision != DDN_PRECISION_FP32_SIMT) {
-    DDN_CHECK_ARG(tc_conv_supported(Cin, Cout, k, stride, pad, dil, H, W), "shape not supported by the tcgen05 path");
+    DDN_CHECK_ARG(tc_conv_supported(Cin, Cout, k, stride, pad, dil, H, W), "shape not supported by the tensor-core path");
     return tc_conv_forward(x, w, y, N, H, W, Cin, Cout, k, stride, pad, dil, precision, (char*)workspace + 3 * wb,
                            workspace_bytes - 3 * wb, st);
   }
@@ -869,9 +871,10 @@ extern "C" int ddn_conv2d_backward(const float* x, const float* w, const float* 
   int Ho = conv_out(H, k, stride, pad, dil), Wo = conv_out(W, k, stride, pad, dil);
   float* wp = (float*)workspace; float* dwp = (float*)((char*)workspace + wb);
   if (precision != DDN_PRECISION_FP32_SIMT) {
-    DDN_CHECK_ARG(tc_conv_supported(Cin, Cout, k, stride, pad, dil, H, W), "shape not supported by the tcgen05 path");
+    DDN_CHECK_ARG(tc_conv_supported(Cin, Cout, k, stride, pad, dil, H, W), "shape not supported by the tensor-core path");
+    // [wb, 3 wb) holds the fp64 weight-gradient accumulator
     return tc_conv_backward(x, w, dy, dx, nullptr, dw, N, H, W, Cin, Cout, k, stride, pad, dil, precision,
-                            (char*)workspace + 3 * wb, workspace_bytes - 3 * wb, dwp, st);
+                            (char*)workspace + 3 * wb, workspace_bytes - 3 * wb, reinterpret_cast<double*>(dwp), st);
   }
   ConvGeom g;
   DDN_TRY(conv_geom_init(&g, N, H, W, Cin, Ho, Wo, Cout, k, k, stride, 1, pad, dil));

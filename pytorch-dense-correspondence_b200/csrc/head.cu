@@ -101,12 +101,13 @@ fc_dgrad_kernel(const float* __restrict__ dlow, const float* __restrict__ w, flo
   }
 }
 
-// dw[d][c] = sum_{n,p} dlow[n][d][p]*feat[n][p][c];  dbias[d] = sum dlow.  Block = C threads-quads x pixel chunk.
+// dw[d][c] = sum_{n,p} dlow[n][d][p]*feat[n][p][c];  dbias[d] = sum dlow.  Block = C threads-quads x pixel chunk; every block
+// stores its partial sums in its own slot of `part` ([D*C] weights, then [D] biases) and fc_part_reduce_kernel adds the slots
+// in a fixed order, so the gradient is the same on every run (no float atomics).
 template <int DM>
 __global__ void __launch_bounds__(256)
 fc_wgrad_kernel(const float* __restrict__ dlow, const float* __restrict__ feat, const __nv_bfloat16* __restrict__ feat_hi,
-                const __nv_bfloat16* __restrict__ feat_lo, float* __restrict__ dw,
-                float* __restrict__ dbias, int64_t Mimg, int N, int C, int D, int pix_per_block) {
+                const __nv_bfloat16* __restrict__ feat_lo, float* __restrict__ part, int64_t Mimg, int N, int C, int D, int pix_per_block) {
   pdl_prologue();
   const int64_t total = (int64_t)N * Mimg;
   const int64_t p0 = (int64_t)blockIdx.x * pix_per_block;
@@ -140,19 +141,32 @@ fc_wgrad_kernel(const float* __restrict__ dlow, const float* __restrict__ feat, 
       for (int d = 0; d < DM; ++d) bsum[d] += g[d];
     }
   }
+  float* slot = part + (size_t)blockIdx.x * (D * C + D);
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
     int c = threadIdx.x + k * 256;
     if (c < C) {
 #pragma unroll
       for (int d = 0; d < DM; ++d)
-        if (d < D) atomicAdd(dw + d * C + c, acc[k][d]);
+        if (d < D) slot[d * C + c] = acc[k][d];
     }
   }
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int d = 0; d < DM; ++d)
-      if (d < D) atomicAdd(dbias + d, bsum[d]);
+      if (d < D) slot[D * C + d] = bsum[d];
+  }
+}
+
+// dw / dbias = the sum of the per-block slots of fc_wgrad_kernel / fc_wgrad_planes_kernel, in block order (fp64)
+__global__ void __launch_bounds__(256)
+fc_part_reduce_kernel(const float* __restrict__ part, int n_slots, int slot_len, int DC, float* __restrict__ dw, float* __restrict__ dbias) {
+  pdl_prologue();
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < slot_len; i += gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int b = 0; b < n_slots; ++b) s += (double)__ldg(part + (size_t)b * slot_len + i);
+    if (i < DC) dw[i] = (float)s;
+    else dbias[i - DC] = (float)s;
   }
 }
 
@@ -251,7 +265,7 @@ int launch_nchw_to_nhwc4(const float* x, float* y, int N, int H, int W, cudaStre
 template <int DM>
 __global__ void __launch_bounds__(256)
 fc_wgrad_planes_kernel(const float* __restrict__ dlow, const __nv_bfloat16* __restrict__ feat_hi, const __nv_bfloat16* __restrict__ feat_lo,
-                       float* __restrict__ dw, float* __restrict__ dbias, int64_t Mimg, int N, int D, int pix_per_block) {
+                       float* __restrict__ part, int64_t Mimg, int N, int D, int pix_per_block) {
   pdl_prologue();
   constexpr int C = 512;
   const int64_t total = (int64_t)N * Mimg;
@@ -299,7 +313,7 @@ fc_wgrad_planes_kernel(const float* __restrict__ dlow, const __nv_bfloat16* __re
       for (int d = 0; d < DM; ++d) bsum[d] += ga[d] + gb[d];
     }
   }
-  // the 4 pixel groups of the block are folded through shared memory one after the other, then one atomic per (d, c)
+  // the 4 pixel groups of the block are folded through shared memory one after the other, then the block's slot is stored
   __shared__ float s_acc[DM][C];
   __shared__ float s_b[4][DM];
   if (cq == 0) {
@@ -323,15 +337,16 @@ fc_wgrad_planes_kernel(const float* __restrict__ dlow, const __nv_bfloat16* __re
     __syncthreads();
   }
   if (rr == 0) {
+    float* slot = part + (size_t)blockIdx.x * (D * C + D);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll
       for (int d = 0; d < DM; ++d)
-        if (d < D) atomicAdd(dw + d * C + cq * 8 + j, acc[j][d]);
+        if (d < D) slot[d * C + cq * 8 + j] = acc[j][d];
     if (cq == 0) {
 #pragma unroll
       for (int d = 0; d < DM; ++d)
-        if (d < D) atomicAdd(dbias + d, s_b[0][d] + s_b[1][d] + s_b[2][d] + s_b[3][d]);
+        if (d < D) slot[D * C + d] = s_b[0][d] + s_b[1][d] + s_b[2][d] + s_b[3][d];
     }
   }
 }
@@ -351,7 +366,7 @@ int launch_fc_forward(const float* feat, const __nv_bfloat16* feat_hi, const __n
 }
 
 int launch_fc_backward(const float* dlow, const float* feat, const __nv_bfloat16* feat_hi, const __nv_bfloat16* feat_lo, const float* w,
-                       float* dfeat, float* dw, float* dbias, int64_t Mimg, int N, int C, int D, cudaStream_t st) {
+                       float* dfeat, float* dw, float* dbias, float* part, int64_t Mimg, int N, int C, int D, cudaStream_t st) {
   DDN_CHECK_ARG(feat || feat_hi, "fc: no feature tensor");
   DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD && C % 4 == 0 && C <= 512, "fc: need 1<=D<=32, C%%4==0, C<=512");
   size_t smem = sizeof(float) * D * C;
@@ -361,18 +376,18 @@ int launch_fc_backward(const float* dlow, const float* feat, const __nv_bfloat16
   DDN_LAUNCH(fc_dgrad_kernel<DM>, ew_blocks(total * (C / 4), 256), 256, smem, st, dlow, w, dfeat, Mimg, N, C, D)
   FC_DISPATCH(D, CALL);
 #undef CALL
-  DDN_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * D * C, st));
-  DDN_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * D, st));
-  int ppb = (int)std::max<int64_t>(16, ceil_div(total, (int64_t)num_sms() * 4));
-  int blocks = (int)ceil_div(total, ppb);
+  const int ppb = (int)std::max<int64_t>(16, ceil_div(total, FC_PART_SLOTS));
+  const int blocks = (int)ceil_div(total, ppb);            // <= FC_PART_SLOTS
   if (!feat && C == 512 && D <= 8) {
-    if (D <= 4) DDN_LAUNCH(fc_wgrad_planes_kernel<4>, blocks, 256, 0, st, dlow, feat_hi, feat_lo, dw, dbias, Mimg, N, D, ppb);
-    else DDN_LAUNCH(fc_wgrad_planes_kernel<8>, blocks, 256, 0, st, dlow, feat_hi, feat_lo, dw, dbias, Mimg, N, D, ppb);
-    return 0;
-  }
-#define CALL(DM) DDN_LAUNCH(fc_wgrad_kernel<DM>, blocks, 256, 0, st, dlow, feat, feat_hi, feat_lo, dw, dbias, Mimg, N, C, D, ppb)
-  FC_DISPATCH(D, CALL);
+    if (D <= 4) DDN_LAUNCH(fc_wgrad_planes_kernel<4>, blocks, 256, 0, st, dlow, feat_hi, feat_lo, part, Mimg, N, D, ppb);
+    else DDN_LAUNCH(fc_wgrad_planes_kernel<8>, blocks, 256, 0, st, dlow, feat_hi, feat_lo, part, Mimg, N, D, ppb);
+  } else {
+#define CALL(DM) DDN_LAUNCH(fc_wgrad_kernel<DM>, blocks, 256, 0, st, dlow, feat, feat_hi, feat_lo, part, Mimg, N, C, D, ppb)
+    FC_DISPATCH(D, CALL);
 #undef CALL
+  }
+  const int slot_len = D * C + D;
+  DDN_LAUNCH(fc_part_reduce_kernel, (int)ceil_div(slot_len, 256), 256, 0, st, part, blocks, slot_len, D * C, dw, dbias);
   return 0;
 }
 

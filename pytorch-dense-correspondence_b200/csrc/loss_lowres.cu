@@ -7,14 +7,16 @@
 // channels are one contiguous 4*D-byte row), and that map -- 0.3*D MB for a batch of 16 -- lives in L2.  So these kernels
 //   forward : read the two indices of a pair from HBM, 2 x 4 low-resolution cells from L2, blend (the same fp32 arithmetic as
 //             upsample_fwd_kernel), squared distance / hinge / count / reduce -- the full-resolution image is never touched;
-//   backward: scatter coef * d(l_j)/d(descriptor) * blend weights straight into d(low) (vector reds into an L2-resident
-//             array), runs of equal A indices folded by a segmented warp reduction first -- no zero-filled full-resolution
-//             gradient, no pass of the upsample backward over it.
+//   backward: scatter coef * d(l_j)/d(descriptor) * blend weights straight into d(low) (fp64 reds into an L2-resident
+//             array, so that the order in which pairs arrive cannot change the fp32 result: a step's gradient is the same
+//             on every run), runs of equal A indices folded by a segmented warp reduction first -- no zero-filled
+//             full-resolution gradient, no pass of the upsample backward over it.
 // HBM traffic per index pair drops from 16 + 8*D algorithmic bytes (and 8 + 64*D bytes of 32-byte sectors actually moved by
 // the channel-strided NCHW gather) to the 16 bytes of the two indices.
 //
 // Descriptor images: low_a / low_b [B, h*w, D] fp32 (what ddn_resnet34_8s_forward writes to `low_nhwc_out`).
 #include <cstdlib>
+#include "bn_stats.cuh"
 #include "loss.cuh"
 
 namespace ddn {
@@ -142,13 +144,9 @@ loss_lowres_fwd_kernel(const float* __restrict__ la, const float* __restrict__ l
   }
 }
 
-__device__ __forceinline__ void red_add_v4f(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-// scatter g[0..D) * blend weights into the 4 cells of pixel `bl` (vector reds when D is a multiple of 4)
+// scatter g[0..D) * blend weights into the 4 cells of pixel `bl` of the fp64 accumulator
 template <int D_T>
-__device__ __forceinline__ void scatter_desc(float* __restrict__ dL, const Blend& bl, int D_rt, const float (&g)[D_T > 0 ? D_T : LOSS_MAXD]) {
+__device__ __forceinline__ void scatter_desc(double* __restrict__ dL, const Blend& bl, int D_rt, const float (&g)[D_T > 0 ? D_T : LOSS_MAXD]) {
   constexpr int DM = D_T > 0 ? D_T : LOSS_MAXD;
   const int D = D_T > 0 ? D_T : D_rt;
   const float wts[4] = {(1.f - bl.lh) * (1.f - bl.lw), (1.f - bl.lh) * bl.lw, bl.lh * (1.f - bl.lw), bl.lh * bl.lw};
@@ -157,15 +155,10 @@ __device__ __forceinline__ void scatter_desc(float* __restrict__ dL, const Blend
   for (int k = 0; k < 4; ++k) {
     const float wk = wts[k];
     if (k > 0 && wk == 0.f) continue;           // clamped edge cells coincide with cell 0 and carry weight 0
-    float* dst = dL + (size_t)cell[k] * D;
-    if (D_T > 0 && D_T % 4 == 0) {
+    double* dst = dL + (size_t)cell[k] * D;
 #pragma unroll
-      for (int q = 0; q < DM / 4; ++q) red_add_v4f(dst + 4 * q, wk * g[4 * q], wk * g[4 * q + 1], wk * g[4 * q + 2], wk * g[4 * q + 3]);
-    } else {
-#pragma unroll
-      for (int c = 0; c < DM; ++c)
-        if (c < D) atomicAdd(dst + c, wk * g[c]);
-    }
+    for (int c = 0; c < DM; ++c)
+      if (c < D) red_add_f64(dst + c, (double)(wk * g[c]));
   }
 }
 
@@ -173,7 +166,7 @@ template <int D_T>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, int D_rt, float sh, float sw,
                        const __grid_constant__ DevTerms T, const float* __restrict__ coef, const float* __restrict__ upstream,
-                       float* __restrict__ dla, float* __restrict__ dlb) {
+                       double* __restrict__ dla, double* __restrict__ dlb) {
   pdl_prologue();
   constexpr int DM = D_T > 0 ? D_T : LOSS_MAXD;
   const int D = D_T > 0 ? D_T : D_rt;
@@ -186,8 +179,8 @@ loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ l
   const int64_t cells = (int64_t)h * w;
   const float* A = la + (size_t)b * cells * D;
   const float* Bq = lb + (size_t)b * cells * D;
-  float* dA = dla + (size_t)b * cells * D;
-  float* dB = dlb + (size_t)b * cells * D;
+  double* dA = dla + (size_t)b * cells * D;
+  double* dB = dlb + (size_t)b * cells * D;
   const int64_t nvalid = tm.len ? min(tm.len[b], tm.n) : tm.n;
   const int64_t j = (int64_t)(blockIdx.x - tm.block_begin) * LR_THREADS + threadIdx.x;
   const int lane = threadIdx.x & 31;
@@ -350,7 +343,7 @@ loss_lowres_fwd_quad_kernel(const float* __restrict__ la, const float* __restric
 }
 
 template <int LPP>
-__device__ __forceinline__ void scatter_quad(float* __restrict__ dL, const Blend& bl, int sub, float4 g) {
+__device__ __forceinline__ void scatter_quad(double* __restrict__ dL, const Blend& bl, int sub, float4 g) {
   constexpr int D = 4 * LPP;
   const float wts[4] = {(1.f - bl.lh) * (1.f - bl.lw), (1.f - bl.lh) * bl.lw, bl.lh * (1.f - bl.lw), bl.lh * bl.lw};
   const int cell[4] = {bl.c00, bl.c01, bl.c10, bl.c11};
@@ -358,7 +351,9 @@ __device__ __forceinline__ void scatter_quad(float* __restrict__ dL, const Blend
   for (int k = 0; k < 4; ++k) {
     const float wk = wts[k];
     if (k > 0 && wk == 0.f) continue;           // clamped edge cells coincide with cell 0 and carry weight 0
-    red_add_v4f(dL + (size_t)cell[k] * D + 4 * sub, wk * g.x, wk * g.y, wk * g.z, wk * g.w);
+    double* dst = dL + (size_t)cell[k] * D + 4 * sub;
+    red_add_f64(dst, (double)(wk * g.x)); red_add_f64(dst + 1, (double)(wk * g.y));
+    red_add_f64(dst + 2, (double)(wk * g.z)); red_add_f64(dst + 3, (double)(wk * g.w));
   }
 }
 
@@ -366,7 +361,7 @@ template <int LPP>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, float sh, float sw,
                             const __grid_constant__ DevTerms T, const float* __restrict__ coef, const float* __restrict__ upstream,
-                            float* __restrict__ dla, float* __restrict__ dlb) {
+                            double* __restrict__ dla, double* __restrict__ dlb) {
   pdl_prologue();
   constexpr int D = 4 * LPP, PPB = LR_THREADS / LPP, PPW = 32 / LPP;      // pairs per block / per warp
   const int b = blockIdx.y;
@@ -378,8 +373,8 @@ loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restric
   const int64_t cells = (int64_t)h * w;
   const float* A = la + (size_t)b * cells * D;
   const float* Bq = lb + (size_t)b * cells * D;
-  float* dA = dla + (size_t)b * cells * D;
-  float* dB = dlb + (size_t)b * cells * D;
+  double* dA = dla + (size_t)b * cells * D;
+  double* dB = dlb + (size_t)b * cells * D;
   const int64_t nvalid = tm.len ? min(tm.len[b], tm.n) : tm.n;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPP, pidx = lane / LPP;
@@ -445,6 +440,12 @@ static int build_terms_lr(const ddn_loss_term* th, int n_terms, DevTerms* T, int
 }
 static float ac_scale(int in, int out) { return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f; }
 
+// dl[i] += (float)acc[i]: the fp64 scatter accumulator into the caller's fp32 gradient
+__global__ void add_f64_to_f32_kernel(const double* __restrict__ acc, float* __restrict__ dl, int64_t n) {
+  pdl_prologue();
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) dl[i] += (float)acc[i];
+}
+
 }  // namespace ddn
 
 using namespace ddn;
@@ -455,7 +456,7 @@ extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const fl
   DDN_TRY(check_common(low_a, low_b, B, (int64_t)H * W, D, W));
   DDN_CHECK_ARG(sums && counts && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null outputs");
   const int lpp = (D == 8 || D == 16 || D == 32) ? D / 4 : 1;
-  // 4 pairs per lane group; 8 (DDN_LOSS_FWD_ITEMS=8) halves the atomics again but costs occupancy: 17.4 -> 18.7-20.9 us at C3
+  // 4 pairs per lane group; 8 (DDN_LOSS_FWD_ITEMS=8) halves the atomics again but costs occupancy
   static const int items = [] { const char* e = getenv("DDN_LOSS_FWD_ITEMS"); return (e && atoi(e) == 8) ? 8 : 4; }();
   DevTerms T;
   DDN_TRY(build_terms_lr(terms_host, n_terms, &T, lpp > 1 ? LR_THREADS / lpp * items : LR_THREADS));
@@ -491,10 +492,10 @@ extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const fl
 extern "C" int ddn_contrastive_terms_backward_lowres(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
                                                      const ddn_loss_term* terms_host, int n_terms,
                                                      const float* coef, const float* upstream,
-                                                     float* dlow_a, float* dlow_b, void* stream) {
+                                                     float* dlow_a, float* dlow_b, double* scratch, void* stream) {
   DDN_TRY(check_common(low_a, low_b, B, (int64_t)H * W, D, W));
-  DDN_CHECK_ARG(coef && dlow_a && dlow_b && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null buffers");
-  DDN_CHECK_ARG(((reinterpret_cast<uintptr_t>(dlow_a) | reinterpret_cast<uintptr_t>(dlow_b) | reinterpret_cast<uintptr_t>(low_a) | reinterpret_cast<uintptr_t>(low_b)) & 15) == 0,
+  DDN_CHECK_ARG(coef && dlow_a && dlow_b && scratch && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null buffers");
+  DDN_CHECK_ARG(((reinterpret_cast<uintptr_t>(dlow_a) | reinterpret_cast<uintptr_t>(dlow_b) | reinterpret_cast<uintptr_t>(scratch) | reinterpret_cast<uintptr_t>(low_a) | reinterpret_cast<uintptr_t>(low_b)) & 15) == 0,
                 "low-resolution maps and their gradients must be 16-byte aligned");
   const int lpp = (D == 8 || D == 16 || D == 32) ? D / 4 : 1;
   DevTerms T;
@@ -504,10 +505,15 @@ extern "C" int ddn_contrastive_terms_backward_lowres(const float* low_a, const f
   dim3 grid(T.total_blocks, B);
   double pairs = 0;
   for (int i = 0; i < n_terms; ++i) pairs += (double)terms_host[i].n * B;
-  ProfScope ps(PROF_LOSS_BWD, pairs * (16.0 + 24.0 * D), st);
+  const int64_t n_low = (int64_t)B * h * w * D;
+  double* dacc_a = scratch;                     // [2][B, h*w, D] fp64: the scatter target, added to dlow_a / dlow_b at the end
+  double* dacc_b = scratch + n_low;
+  DDN_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * 2 * (size_t)n_low, st));
   const float sh = ac_scale(h, H), sw = ac_scale(w, W);
-#define BWD(DT) DDN_LAUNCH(loss_lowres_bwd_kernel<DT>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, coef, upstream, dlow_a, dlow_b)
-#define BWDQ(L) DDN_LAUNCH(loss_lowres_bwd_quad_kernel<L>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, coef, upstream, dlow_a, dlow_b)
+  {
+  ProfScope ps(PROF_LOSS_BWD, pairs * (16.0 + 24.0 * D), st);
+#define BWD(DT) DDN_LAUNCH(loss_lowres_bwd_kernel<DT>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, coef, upstream, dacc_a, dacc_b)
+#define BWDQ(L) DDN_LAUNCH(loss_lowres_bwd_quad_kernel<L>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, coef, upstream, dacc_a, dacc_b)
   switch (D) {
     case 3: BWD(3); break;
     case 4: BWD(4); break;
@@ -518,5 +524,9 @@ extern "C" int ddn_contrastive_terms_backward_lowres(const float* low_a, const f
   }
 #undef BWD
 #undef BWDQ
+  }
+  const int blocks = (int)std::min<int64_t>(ceil_div(n_low, 256), (int64_t)num_sms() * 8);
+  DDN_LAUNCH(add_f64_to_f32_kernel, blocks, 256, 0, st, dacc_a, dlow_a, n_low);
+  DDN_LAUNCH(add_f64_to_f32_kernel, blocks, 256, 0, st, dacc_b, dlow_b, n_low);
   return 0;
 }

@@ -24,7 +24,7 @@ def init_from_env(backend=None):
             backend = "nccl" if torch.cuda.is_available() else "gloo"
         if backend == "nccl":
             torch.cuda.set_device(local_rank)
-            # Experiments, both off by default (profiles/r2_reserved_sms_ab.md): DDN_OVERLAP_RESERVED_SMS=n keeps n SMs free of the
+            # Experiments, both off by default (not measured on H100): DDN_OVERLAP_RESERVED_SMS=n keeps n SMs free of the
             # persistent kernels from the first gradient bucket to the end of the backward, DDN_RESERVED_SMS=n for the whole step;
             # NCCL is then capped at n CTAs so that it fits there.
             cap = max(int(os.environ.get("DDN_OVERLAP_RESERVED_SMS", "0")), int(os.environ.get("DDN_RESERVED_SMS", "0")))

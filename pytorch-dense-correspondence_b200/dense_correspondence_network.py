@@ -157,7 +157,7 @@ class DenseCorrespondenceNetwork(nn.Module):
 
     @staticmethod
     def get_unet(config):
-        raise NotImplementedError("the Unet backbone is not part of the B200 hot path (net.py:346-357)")
+        raise NotImplementedError("the Unet backbone is not part of this hot path (net.py:346-357)")
 
     @staticmethod
     def get_fcn(config):
@@ -165,7 +165,7 @@ class DenseCorrespondenceNetwork(nn.Module):
         if config["backbone"]["model_class"] == "Resnet":
             resnet_model = config["backbone"]["resnet_name"]
             if not hasattr(resnet_dilated, resnet_model):
-                raise ValueError("backbone %s is not implemented in the B200 path (only Resnet34_8s)" % resnet_model)
+                raise ValueError("backbone %s is not implemented in this path (only Resnet34_8s)" % resnet_model)
             fcn = getattr(resnet_dilated, resnet_model)(num_classes=config['descriptor_dimension'])
         elif config["backbone"]["model_class"] == "Unet":
             fcn = DenseCorrespondenceNetwork.get_unet(config)

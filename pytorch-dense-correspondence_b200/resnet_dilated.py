@@ -7,7 +7,7 @@ on top of .../vision/torchvision/models/resnet.py:112-265).
 Same constructor, same ``forward(x, feature_alignment=False)``, same 218 state-dict keys
 (``resnet34_8s.conv1.weight`` ... ``resnet34_8s.fc.bias``), same train()/eval() BatchNorm semantics --
 but the module holds no torch.nn layers: all learnable tensors are views into one flat fp32 array
-and the whole forward / backward runs inside libddn_b200.so (hand-written sm_100a kernels) through
+and the whole forward / backward runs inside libddn_b200.so (hand-written sm_90a kernels) through
 one autograd.Function.  CUDA only; there is no CPU path.
 
 Differences from the reference constructor, on purpose: no ImageNet download (``pretrained=True`` at
@@ -31,7 +31,7 @@ _default_precision = [N.PRECISION_BF16X3]     # fp32-equivalent results on the t
 
 
 def set_default_precision(p):
-    """'bf16x3' (tcgen05, operands split hi+lo: fp32-equivalent results, the default) or 'bf16' (tcgen05 single pass: fast,
+    """'bf16x3' (wgmma, operands split hi+lo: fp32-equivalent results, the default) or 'bf16' (wgmma single pass: fast,
     fails the 1e-3 descriptor gate).  There is ONE execution path -- the tensor cores; the fp32 CUDA-core kernels that the
     library also contains are a parity instrument of the test-suite, not a backend, and are refused unless
     DDN_TEST_FP32_SIMT=1 is set (tests/conftest.py sets it)."""
@@ -325,7 +325,7 @@ class Resnet34_8s(nn.Module):
                                                        (self._wcache_nonce << 20) + self._flat_version, prec))
 
     def mark_parameters_changed(self):
-        """Kept for callers of round 1: a no-op now (parameter changes are detected on the device)."""
+        """Kept for existing callers: a no-op now (parameter changes are detected on the device)."""
 
     @property
     def flat_gradient(self):

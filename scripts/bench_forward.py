@@ -3,9 +3,9 @@ SURVEY.md 8d "forward-only target": imgs/s x 211.909 GFLOP / peak).
 
 Rows: train-mode BN (batch statistics from the conv epilogue + one BN-apply pass per conv) and eval-mode BN (inference:
 BN + residual + ReLU folded into the conv epilogue, dense_correspondence_network.py:265-299 forward_single_image_tensor /
-evaluation).  Images are resident in HBM; whole forward timed with CUDA events on the current stream, the tcgen05 conv
+evaluation).  Images are resident in HBM; whole forward timed with CUDA events on the current stream, the tensor-core conv
 launches additionally timed one by one through ddn_profile_* (a separate pass, so the per-launch events do not perturb
-the headline).  Prints one JSON object; run on the GPU box."""
+the headline).  Prints one JSON object; needs a GPU."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -15,7 +15,7 @@ from pdc_b200 import _native as N
 
 pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
 peaks = json.load(open(pk)) if os.path.exists(pk) else {}
-peak_tf = float(peaks.get("bf16_tflops_sustained", 1441.5))
+peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))      # else the H100 SXM data sheet, dense bf16
 B, D, H, W = int(os.environ.get("FWD_BATCH", "16")), 3, 480, 640
 GF_IMG = 211.909
 steps, warmup = int(os.environ.get("FWD_STEPS", "20")), int(os.environ.get("FWD_WARMUP", "5"))

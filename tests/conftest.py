@@ -13,7 +13,7 @@ os.environ.setdefault("DDN_TEST_FP32_SIMT", "1")      # the fp32 CUDA-core kerne
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with `-m gpu`)")
     # the GPU boxes advertise 128 logical CPUs to a throttled container: 128 torch threads make the CPU oracle ~50x slower
     import torch
     torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))

@@ -27,7 +27,7 @@ def test_header_symbols_exported_and_bound():
     for n in names:
         assert hasattr(lib, n), "declared in ddn_b200.h but not exported: " + n
     assert set(names) == set(N.EXPORTED_SYMBOLS), set(names) ^ set(N.EXPORTED_SYMBOLS)
-    assert N.lib.ddn_abi_version() == 2
+    assert N.lib.ddn_abi_version() == 3
 
 
 @pytest.mark.parametrize("D", [3, 8, 16])

@@ -72,11 +72,11 @@ TC_CASES = [c for c in CONV_CASES if c[6] == 1] + [
 @pytest.mark.parametrize("precision,tol", [("bf16x3", 2e-5), ("bf16", 8e-3)])
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv2d_tcgen05(case, precision, tol):
-    """tcgen05 implicit GEMM vs the fp32 CPU reference: bf16x3 split must be fp32-class (<= 2e-5 relative Frobenius
+    """wgmma implicit GEMM vs the fp32 CPU reference: bf16x3 split must be fp32-class (<= 2e-5 relative Frobenius
     error, ~2^-16 per product), single-pass bf16 within bf16 rounding."""
     prec = {"bf16x3": N.PRECISION_BF16X3, "bf16": N.PRECISION_BF16}[precision]
     if N.lib.ddn_resnet34_8s_workspace_bytes(1, 64, 64, 3, 1, prec) == 0:
-        pytest.skip("tcgen05 path not in this build")
+        pytest.skip("tensor-core path not in this build")
     n, h, w, cin, cout, k, s, p, d = case
     g = torch.Generator().manual_seed(hash(case) % 1000 + 1)
     x = torch.randn(n, cin, h, w, generator=g)
@@ -384,7 +384,7 @@ def test_device_reprojection_match_finder_vs_restated_reference():
         assert float((gu2.cpu() - ref_b[0]).abs().max()) < 2e-2 and float((gv2.cpu() - ref_b[1]).abs().max()) < 2e-2
 
 
-# ---------------------------------------------------------------------------------------------------- round 2
+# ----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("over", [{}, {"scale_by_hard_negatives": False},
                                   {"use_l2_pixel_loss_on_masked_non_matches": True, "use_l2_pixel_loss_on_background_non_matches": True, "M_pixel": 9}])
 def test_ragged_batch_matches_the_reference_loop(over):

@@ -1,5 +1,6 @@
-"""CPU: the oracle restatements are pinned against the EXECUTED reference source (oracle/_ref, generated by
-oracle/build_ref.py from /root/reference with documented line-anchored py2->py3 patches):
+"""CPU: the oracle restatements are pinned against what the EXECUTED reference source computed (oracle/make_golden.py runs
+the reference's own files -- oracle/build_ref.py: documented line-anchored py2->py3 patches -- on the cases of
+oracle/ref_cases.py and stores the results in tests/golden/reference_checks.npz and tests/golden/loss_*.npz):
 
   * loss: values, hard-negative counts and autograd gradients of PixelwiseContrastiveLoss.* and loss_composer.*
     (dense_correspondence/loss_functions/pixelwise_contrastive_loss.py:35-411, loss_composer.py:7-218)
@@ -7,27 +8,31 @@ oracle/build_ref.py from /root/reference with documented line-anchored py2->py3 
     (correspondence_tools/correspondence_finder.py:276-405, dataset/spartan_dataset_masked.py:841-858,1255-1264)
   * reprojection match finder: batch_find_pixel_correspondences (correspondence_finder.py:409-619)
 
-and the committed golden loss vectors are the executed reference's outputs.  Skipped where neither /root/reference nor a
-prebuilt oracle/_ref exists."""
+The generator requires the restatement to equal the reference bit-for-bit; here integer results must match exactly and
+floating-point ones to ~1 ulp, because a different CPU can reorder a vectorised fp32 reduction."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import build_ref
 from oracle import loss_oracle as LO
+from oracle import ref_cases as RC
 from oracle.resnet34_8s_oracle import process_network_output
-
-pytestmark = pytest.mark.skipif(not (build_ref.reference_available() or build_ref.ref_built()),
-                                reason="needs /root/reference (build container) or a prebuilt oracle/_ref")
 
 
 @pytest.fixture(scope="module")
-def ref():
-    if build_ref.reference_available():
-        build_ref.build()          # always regenerate from the tree that is present
-    return build_ref.load()
+def stored(golden_dir):
+    return np.load(os.path.join(golden_dir, "reference_checks.npz"))
+
+
+def assert_same_result(got, want, what, rtol=1e-6, atol=1e-7):
+    assert got.shape == want.shape, what
+    if np.issubdtype(want.dtype, np.floating):
+        assert got.dtype == want.dtype, what
+        np.testing.assert_allclose(got, want, rtol=rtol, atol=atol, err_msg=what)
+    else:
+        assert np.array_equal(got, want), what
 
 
 def _golden_case(golden_dir, name):
@@ -52,158 +57,57 @@ def _run(pcl, get_loss, A, B, idx, match_type=0):
 
 
 @pytest.mark.parametrize("name", ["loss_default_d3", "loss_pixelw_blind_d8", "loss_noscale_d16"])
-def test_composed_loss_restatement_equals_executed_reference(ref, golden_dir, name):
+def test_composed_loss_restatement_equals_executed_reference(golden_dir, name):
+    # the committed goldens ARE the executed reference's outputs (oracle/make_golden.py writes them from it)
     g, cfg, idx = _golden_case(golden_dir, name)
     A, B = torch.tensor(g["A"]), torch.tensor(g["B"])
     _, D, H, W = A.shape
-    five_r, dA_r, dB_r = _run(ref.pcl.PixelwiseContrastiveLoss([H, W], dict(cfg)), ref.composer.get_loss, A, B, idx)
     five_o, dA_o, dB_o = _run(LO.TorchPixelwiseContrastiveLoss([H, W], dict(cfg)), LO.get_loss, A, B, idx)
-    assert five_o == five_r                                    # same torch ops in the same order: bit-equal
-    assert torch.equal(dA_o, dA_r) and torch.equal(dB_o, dB_r)
-    # the committed goldens ARE the executed reference's outputs (oracle/make_golden.py writes them from it)
-    np.testing.assert_allclose(five_r, g["five"], rtol=1e-6, atol=1e-8)
-    np.testing.assert_allclose(dA_r.numpy(), g["dA"], rtol=1e-5, atol=1e-8)
-    np.testing.assert_allclose(dB_r.numpy(), g["dB"], rtol=1e-5, atol=1e-8)
+    np.testing.assert_allclose(five_o, g["five"], rtol=1e-6, atol=1e-8)
+    np.testing.assert_allclose(dA_o.numpy(), g["dA"], rtol=1e-5, atol=1e-8)
+    np.testing.assert_allclose(dB_o.numpy(), g["dB"], rtol=1e-5, atol=1e-8)
 
 
-def test_every_loss_method_equals_executed_reference(ref):
-    H, W, D, P = 12, 20, 5, 240
-    gen = torch.Generator().manual_seed(3)
-    A = 0.3 * torch.randn(1, P, D, generator=gen); B = 0.3 * torch.randn(1, P, D, generator=gen)
-    ma = torch.randint(0, P, (7,), generator=gen); mb = torch.randint(0, P, (7,), generator=gen)
-    na = ma.repeat_interleave(4); nb = torch.randint(0, P, (28,), generator=gen)
-    cfg = dict(LO.DEFAULT_LOSS_CONFIG, M_descriptor=0.6)
-    r = ref.pcl.PixelwiseContrastiveLoss([H, W], dict(cfg)); o = LO.TorchPixelwiseContrastiveLoss([H, W], dict(cfg))
-
-    def same(x, y):
-        if isinstance(x, torch.Tensor):
-            assert x.shape == y.shape and torch.equal(x, y)
-        elif isinstance(x, (tuple, list)):
-            assert len(x) == len(y)
-            for a, b in zip(x, y):
-                same(a, b)
-        else:
-            assert x == y
-
-    same(o.match_loss(A, B, ma, mb), r.match_loss(A, B, ma, mb))
-    for inv in (False, True):
-        same(o.non_match_descriptor_loss(A, B, na, nb, M=0.6, invert=inv), r.non_match_descriptor_loss(A, B, na, nb, M=0.6, invert=inv))
-        same(o.non_match_loss_descriptor_only(A, B, na, nb, M_descriptor=0.6, invert=inv),
-             r.non_match_loss_descriptor_only(A, B, na, nb, M_descriptor=0.6, invert=inv))
-    same(o.non_match_loss_with_l2_pixel_norm(A, B, mb, na, nb, M_descriptor=0.6, M_pixel=7),
-         r.non_match_loss_with_l2_pixel_norm(A, B, mb, na, nb, M_descriptor=0.6, M_pixel=7))
-    same(o.l2_pixel_loss(mb, nb, M_pixel=7), r.l2_pixel_loss(mb, nb, M_pixel=7))
-    same(o.flattened_pixel_locations_to_u_v(nb.unsqueeze(1)), r.flattened_pixel_locations_to_u_v(nb.unsqueeze(1)))
-    for l2 in (False, True):
-        same(o.get_loss_matched_and_non_matched_with_l2(A, B, ma, mb, na, nb, use_l2_pixel_loss=l2),
-             r.get_loss_matched_and_non_matched_with_l2(A, B, ma, mb, na, nb, use_l2_pixel_loss=l2))
-    same(o.get_triplet_loss(A, B, ma, mb, na, nb, 0.1), r.get_triplet_loss(A, B, ma, mb, na, nb, 0.1))
-    same(o.get_loss_original(A, B, ma, mb, na, nb), r.get_loss_original(A, B, ma, mb, na, nb))
-    # single-element index tensors (the unsqueeze branch, pcl.py:161-163,199-201) and identical descriptors (d = 0)
-    one, two = torch.tensor([7]), torch.tensor([11])
-    same(o.match_loss(A, B, one, two), r.match_loss(A, B, one, two))
-    same(o.non_match_descriptor_loss(A, B, one, two, M=100.0), r.non_match_descriptor_loss(A, B, one, two, M=100.0))
-    Z = torch.zeros(1, P, D)
-    same(o.non_match_loss_descriptor_only(Z, Z, na, nb, M_descriptor=0.5), r.non_match_loss_descriptor_only(Z, Z, na, nb, M_descriptor=0.5))
+def test_every_loss_method_equals_executed_reference(stored):
+    got = RC.every_loss_method(LO.TorchPixelwiseContrastiveLoss)
+    want = {k[len("method/"):]: stored[k] for k in stored.files if k.startswith("method/")}
+    assert sorted(got) == sorted(want)
+    for k in want:
+        assert_same_result(got[k], want[k], k)
 
 
-def test_composer_branches_equal_executed_reference(ref):
-    H, W, D, P = 10, 16, 3, 160
-    gen = torch.Generator().manual_seed(9)
-    A = 0.3 * torch.randn(1, D, H, W, generator=gen); B = 0.3 * torch.randn(1, D, H, W, generator=gen)
-    ma = torch.randint(0, P, (6,), generator=gen); mb = torch.randint(0, P, (6,), generator=gen)
-    idx = dict(matches_a=ma, matches_b=mb, masked_a=ma.repeat_interleave(3), masked_b=torch.randint(0, P, (18,), generator=gen),
-               background_a=ma.repeat_interleave(2), background_b=torch.randint(0, P, (12,), generator=gen),
-               blind_a=torch.randint(0, P, (9,), generator=gen), blind_b=torch.randint(0, P, (9,), generator=gen))
-    for over in ({}, {"scale_by_hard_negatives": False}, {"scale_by_hard_negatives_DIFFERENT_OBJECT": False},
-                 {"M_masked": 1e-6, "M_background": 1e-6}):            # the last: zero hard negatives -> max(h, 1)
-        cfg = dict(LO.DEFAULT_LOSS_CONFIG); cfg.update(over)
-        for mt in (0, 2, 3, 4):                                          # within-scene, different-object, multi, synthetic multi
-            five_r, dA_r, dB_r = _run(ref.pcl.PixelwiseContrastiveLoss([H, W], dict(cfg)), ref.composer.get_loss, A, B, idx, mt)
-            five_o, dA_o, dB_o = _run(LO.TorchPixelwiseContrastiveLoss([H, W], dict(cfg)), LO.get_loss, A, B, idx, mt)
-            assert five_o == five_r, (over, mt)
-            assert torch.equal(dA_o, dA_r) and torch.equal(dB_o, dB_r), (over, mt)
-    # blind sentinel [-1]: not entered; across-scene: the reference's own NameError; unknown type: ValueError
-    idx_e = dict(idx, blind_a=ref.dataset.SpartanDataset.empty_tensor(), blind_b=ref.dataset.SpartanDataset.empty_tensor())
-    cfg = dict(LO.DEFAULT_LOSS_CONFIG)
-    five_r, _, _ = _run(ref.pcl.PixelwiseContrastiveLoss([H, W], dict(cfg)), ref.composer.get_loss, A, B, idx_e, 0)
-    five_o, _, _ = _run(LO.TorchPixelwiseContrastiveLoss([H, W], dict(cfg)), LO.get_loss, A, B, idx_e, 0)
-    assert five_o == five_r and five_r[4] == 0.0
-    assert torch.equal(LO.empty_tensor(), ref.dataset.SpartanDataset.empty_tensor())
-    for mod_pcl, mod_get in ((ref.pcl.PixelwiseContrastiveLoss, ref.composer.get_loss), (LO.TorchPixelwiseContrastiveLoss, LO.get_loss)):
-        with pytest.raises((NameError, UnboundLocalError)):
-            _run(mod_pcl([H, W], dict(cfg)), mod_get, A, B, idx, 1)
-        with pytest.raises(ValueError):
-            _run(mod_pcl([H, W], dict(cfg)), mod_get, A, B, idx, 9)
-    T, Tr = LO.SpartanDatasetDataType, ref.dataset.SpartanDatasetDataType
-    assert all(getattr(T, k) == getattr(Tr, k) for k in dir(Tr) if k.isupper())
+def test_composer_branches_equal_executed_reference(stored):
+    """every configuration x match type, the blind sentinel [-1] (not entered), max(h, 1), and the reference's own
+    NameError (across-scene) / ValueError (unknown type)."""
+    got = RC.composer_branches(LO.TorchPixelwiseContrastiveLoss, LO.get_loss, LO.empty_tensor)
+    want = {k[len("composer/"):]: stored[k] for k in stored.files if k.startswith("composer/")}
+    assert sorted(got) == sorted(want)
+    for k in want:
+        assert_same_result(got[k], want[k], k)
+    assert float(got["sentinel/five"][4]) == 0.0
+    assert str(want["raises/across_scene"]) in ("NameError", "UnboundLocalError") and str(want["raises/unknown"]) == "ValueError"
+    T = LO.SpartanDatasetDataType
+    types = [k for k in stored.files if k.startswith("datatype/")]
+    assert types and all(getattr(T, k[len("datatype/"):]) == int(stored[k]) for k in types)
 
 
-def test_non_match_sampler_restatement_equals_executed_reference(ref, monkeypatch):
-    """create_non_correspondences draws torch.rand(n) (mask branch) or torch.rand(2, n) (no mask), then two more draws for the
-    no-op perturbation; the restatement takes the uniforms as arguments -- feed both the same numbers."""
-    H, W, k = 30, 40, 5
-    gen = torch.Generator().manual_seed(4)
-    ma = torch.randint(0, H * W, (11,), generator=gen)
-    uv_a = (ma % W, ma // W)
-    uv_b = ((ma % W).float(), (ma // W).float())
-    n = len(ma) * k
-    ru, rv = torch.rand(n, generator=gen), torch.rand(n, generator=gen)
-    mask = torch.zeros(H, W); mask[5:20, 8:30] = 1.0
-    for m in (mask, None, torch.zeros(H, W)):
-        calls = []
-
-        def fake_rand(*shape):
-            calls.append(shape)
-            if len(calls) == 1:
-                return ru.clone() if shape == (n,) else torch.stack((ru, rv)).clone()
-            return torch.zeros(*shape)
-        monkeypatch.setattr(ref.finder.torch, "rand", fake_rand)
-        try:
-            uv_b_non = ref.finder.create_non_correspondences(uv_b, (H, W), num_non_matches_per_match=k, img_b_mask=m)
-        finally:
-            monkeypatch.undo()
-        SD = ref.dataset.SpartanDataset
-        uv_a_long, uv_b_long = SD.create_non_matches(None, uv_a, uv_b_non, k)
-        na_r = SD.flatten_uv_tensor(uv_a_long, W).squeeze(1); nb_r = SD.flatten_uv_tensor(uv_b_long, W).squeeze(1)
+def test_non_match_sampler_restatement_equals_executed_reference(stored):
+    """The reference sampler was given the same uniform numbers the restatement takes as arguments."""
+    H, W, k, ma, ru, rv, masks = RC.sampler_inputs()
+    for i, m in enumerate(masks):
         na_o, nb_o = LO.create_non_correspondences_flat(ma, (H, W), k, m, ru, rv)
-        assert torch.equal(na_o, na_r) and torch.equal(nb_o, nb_r)
-        if m is mask:
-            assert bool((mask.view(-1)[nb_r] == 1).all())
+        assert_same_result(na_o.numpy(), stored["sampler/%d/a" % i], "sampler %d a" % i)
+        assert_same_result(nb_o.numpy(), stored["sampler/%d/b" % i], "sampler %d b" % i)
+        if i == 0:
+            assert bool((m.view(-1)[nb_o] == 1).all())
 
 
-def test_reprojection_restatement_equals_executed_reference(ref, monkeypatch):
-    H, W, n = 120, 160, 900
-    K = np.array([[133.4, 0, 79.8], [0, 133.7, 59.1], [0, 0, 1.0]])
-
-    def pose(rx, ry, t):
-        cx, sx, cy, sy = np.cos(rx), np.sin(rx), np.cos(ry), np.sin(ry)
-        Rx = np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]); Ry = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
-        T = np.eye(4); T[:3, :3] = Ry.dot(Rx); T[:3, 3] = t
-        return T
-    pa, pb = pose(0.01, -0.02, [0, 0, 0]), pose(-0.04, 0.1, [0.15, -0.03, 0.04])
-    nrm, d0 = np.array([-0.1, 0.05, 1.0]), 1.2
-
-    def render(T):
-        us, vs = np.meshgrid(np.arange(W), np.arange(H))
-        rays = np.linalg.inv(K).dot(np.stack([us.ravel(), vs.ravel(), np.ones(H * W)]))
-        s = (d0 - nrm.dot(T[:3, 3])) / nrm.dot(T[:3, :3].dot(rays))
-        return (s * 1000.0).reshape(H, W)
-    da = np.round(render(pa)).astype(np.uint16); db = np.round(render(pb)).astype(np.uint16)
-    da[10:30, 20:50] = 0                                               # no-return pixels (depth 0) are pruned
-    db[60:80, 100:130] = 300                                           # an occluder in front of the plane in image b
-    mask = np.zeros((H, W), dtype=np.float32); mask[5:110, 10:150] = 1.0
-    ru = torch.rand(n, generator=torch.Generator().manual_seed(8))
-    # the reference first draws (and discards) rand(2, n) for unmasked candidates, then rand(n) for the masked sample
-    monkeypatch.setattr(ref.finder.torch, "rand", lambda *s: ru.clone() if s == (n,) else torch.zeros(*s))
-    try:
-        uv_a_r, uv_b_r = ref.finder.batch_find_pixel_correspondences(da, pa, db, pb, num_attempts=n, img_a_mask=mask, K=K)
-    finally:
-        monkeypatch.undo()
+def test_reprojection_restatement_equals_executed_reference(stored):
+    da, pa, db, pb, mask, ru, K, n = RC.reprojection_scene()
     # the candidates random_sample_from_masked_image_torch drew (correspondence_finder.py:92-121)
     nz = torch.nonzero(torch.from_numpy(mask).view(-1))
     cand = torch.index_select(nz, 0, torch.floor(ru * len(nz)).long()).squeeze(1)
     uv_a_o, uv_b_o = LO.batch_find_pixel_correspondences(da, pa, db, pb, cand, K)
-    assert len(uv_a_r[0]) > 0.3 * n and len(uv_a_r[0]) < n              # some pruned by every rule
-    for t_o, t_r in zip(uv_a_o + uv_b_o, uv_a_r + uv_b_r):
-        assert t_o.shape == t_r.shape and torch.equal(t_o, t_r)
+    assert len(stored["reprojection/0"]) > 0.3 * n and len(stored["reprojection/0"]) < n      # some pruned by every rule
+    for i, t in enumerate(uv_a_o + uv_b_o):
+        assert_same_result(t.numpy(), stored["reprojection/%d" % i], "reprojection %d" % i)
