@@ -214,8 +214,9 @@ constexpr int EPI_ROWS = 4;                      // rows per lane group
 constexpr int EPI_STRIDE = 40;                   // floats per staging row: conflict-free float2 writes and float4 reads
 constexpr int EPI_WARP_FLOATS = 16 * EPI_STRIDE;
 
+// the warp's 16 rows x columns 32c .. 32c + 31 of the accumulator -> st[row * EPI_STRIDE + column - 32c]
 template <int K>
-__device__ __forceinline__ void stage_chunk(const float (&acc)[K], int c, float* st, int lane, float4 (&v)[EPI_ROWS]) {
+__device__ __forceinline__ void stage_write(const float (&acc)[K], int c, float* st, int lane) {
   const int r = lane >> 2, q = (lane & 3) * 2;
 #pragma unroll
   for (int jj = 0; jj < 4; ++jj) {
@@ -224,6 +225,11 @@ __device__ __forceinline__ void stage_chunk(const float (&acc)[K], int c, float*
     *reinterpret_cast<float2*>(st + (r + 8) * EPI_STRIDE + 8 * jj + q) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
   }
   __syncwarp();
+}
+
+template <int K>
+__device__ __forceinline__ void stage_chunk(const float (&acc)[K], int c, float* st, int lane, float4 (&v)[EPI_ROWS]) {
+  stage_write(acc, c, st, lane);
   const int ga = lane >> 3, gb = lane & 7;
 #pragma unroll
   for (int i = 0; i < EPI_ROWS; ++i) v[i] = *reinterpret_cast<const float4*>(st + (EPI_ROWS * ga + i) * EPI_STRIDE + 4 * gb);
@@ -399,24 +405,28 @@ __device__ __forceinline__ TcSub tc_sub(const TcConvParams& p, int st) {
 
 // The k-loop of one item whose tile is W channels wide (BLOCK_N, or a tail piece of 64 or 32 channels): acc / accx are the first
 // W columns of the accumulators.  One instantiation per width keeps the accumulator registers of every wgmma in the loop fixed.
-template <int W, int BLOCK_N, int NPROD, int STAGES>
+// TRANS = 0: K-major operands (a k16 step is 32 bytes along the swizzle row).  TRANS = 1: MN-major operands, the weight
+// gradient's 64-pixel boxes of 64 channels (a k16 step is 16 pixel rows, LBO = the next box of 64 channels).
+template <int W, int BLOCK_N, int NPROD, int STAGES, int TRANS = 0>
 __device__ __forceinline__ void conv_tc_mainloop(float (&acc)[W / 2], float (&accx)[W / 2], int num_kb, uint32_t& g, const uint64_t* full_bar,
                                                  const uint64_t* empty_bar, const uint8_t* smem, int wg, int lane) {
   constexpr int NSPLIT = NPROD == 3 ? 2 : 1;
   constexpr int A_BYTES = 128 * TC_BLOCK_K * 2;
   constexpr int B_BYTES = BLOCK_N * TC_BLOCK_K * 2;
   constexpr int STAGE_BYTES = NSPLIT * (A_BYTES + B_BYTES);
+  constexpr uint32_t LBO = TRANS ? TC_SUB_BYTES : 16;
+  constexpr int K_STEP = TRANS ? 16 * 128 : 32;
   for (int kb = 0; kb < num_kb; ++kb, ++g) {
     const int s = g % STAGES;
     mbar_wait(smem_u32(&full_bar[s]), (g / STAGES) & 1);
     wgmma_fence();
     const uint32_t stg = smem_u32(smem + (size_t)s * STAGE_BYTES);
-    const uint64_t a_hi = gmma_desc_k(stg + wg * TC_SUB_BYTES), a_lo = gmma_desc_k(stg + A_BYTES + wg * TC_SUB_BYTES);
-    const uint64_t b_hi = gmma_desc_k(stg + NSPLIT * A_BYTES), b_lo = gmma_desc_k(stg + 2 * A_BYTES + B_BYTES);
+    const uint64_t a_hi = gmma_desc(stg + wg * TC_SUB_BYTES, LBO, 1024), a_lo = gmma_desc(stg + A_BYTES + wg * TC_SUB_BYTES, LBO, 1024);
+    const uint64_t b_hi = gmma_desc(stg + NSPLIT * A_BYTES, LBO, 1024), b_lo = gmma_desc(stg + 2 * A_BYTES + B_BYTES, LBO, 1024);
 #pragma unroll
     for (int k = 0; k < TC_BLOCK_K / 16; ++k) {
-      const uint64_t adv = (uint64_t)((k * 32) >> 4);       // 16 bf16 = 32 bytes along K inside the swizzle row
-      mma_k16_x<W, 0, NPROD>(acc, accx, a_hi + adv, a_lo + adv, b_hi + adv, b_lo + adv, (kb | k) != 0);
+      const uint64_t adv = (uint64_t)((k * K_STEP) >> 4);
+      mma_k16_x<W, TRANS, NPROD>(acc, accx, a_hi + adv, a_lo + adv, b_hi + adv, b_lo + adv, (kb | k) != 0);
     }
     wgmma_commit();
     wgmma_wait<1>();                                    // the previous k-block's MMAs are done: release its slot
@@ -776,161 +786,130 @@ conv64_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
 // dimension.  Both operands are the same NHWC bf16 planes the forward reads, consumed as MN-MAJOR operands
 // (channels contiguous, pixels = K rows), so no transposed copy exists anywhere:
 //   A = dY patch: 64 pixels (4x16) x 128 output channels = two TMA boxes {64 c, 16 w, 4 h, 1 n}, 8 KB each
-//   B = X  patch: 64 shifted pixels x BN input channels   = BN/64 boxes at (w0+(s-1)dil, h0+(r-1)dil); OOB zero fill
-//                                                            is the padding, the shift only touches the W/H coordinates
+//   B = X  patch: the 64 pixels shifted by the tap x BN input channels = BN/64 boxes at (w0+(s-1)dil, h0+(r-1)dil); OOB zero
+//                 fill is the padding, the shift only touches the W/H coordinates
 // In shared memory a box is 64 rows (pixels) of 128 swizzled bytes (64 channels): the canonical MN-major SWIZZLE_128B
-// layout with SBO = 1024 B (next 8 pixels) and LBO = 8192 B (next 64 channels = next box).
-// One CTA owns (128 co) x (BN ci) x (T taps of one filter row) and a contiguous range of pixel patches (split-K); consumer
-// warpgroup wg holds output channels co0 + 64wg .. + 63 of the T accumulators in registers (T * BN / 2 floats per thread,
-// hence BN = 64 for T = 3) and adds them into dwp[tap][co][ci] at the end.  dwp is fp64: the split-K partial sums then
-// arrive in any order and still round to the same fp32 gradient, so a step computes the same weight gradients every run.
-// Two smem rings: A (shared by the T taps of a k-block) and B (one slot per tap).
+// layout with SBO = 1024 B (next 8 pixels) and LBO = 8192 B (next 64 channels = next box).  The stage ring {A_hi, A_lo, B_hi,
+// B_lo} and the k-loop are conv_tc_kernel's (conv_tc_mainloop, TRANS = 1): consumer warpgroup wg issues wgmma.m64nBNk16 for
+// output channels co0 + 64wg .. + 63, the two small bf16x3 products into their own accumulator.
+// A tile is 128 co x BN ci x ONE tap (BN = 128 when Cin % 128 == 0, else 64), so 3x3 and 1x1 convolutions share one path.
+// Work item = (pixel chunk c, tile), numbered chunk-major (item = c * n_tiles + tile) and dealt round-robin to a persistent
+// grid: the CTAs running at one time walk the same pixel range, so the tiles that read a k-block find it in L2.  The host
+// picks the chunk count (tc_wgrad_chunks).  At the end of an item each warp adds its fp32 partial into dwp[tap][co][ci] with
+// fp64 reds, staged through shared memory so that one red instruction covers 32 consecutive doubles of a row; the producer
+// meanwhile loads the next item's stages.  dwp is fp64 and zero-filled: the partial sums arrive in any order and still round
+// to the same fp32 gradient, so a step computes the same weight gradients every run.
 struct TcWgradParams {
   double* dwp;           // [taps][Cout][Cin] fp64, zero-filled by the caller
-  int N, H, W, Cin, Cout;
+  int N, H, W, Cin, Cout;   // H, W: OUTPUT (dY) size
   int taps_w, dil, stride;
   int tiles_h, tiles_w;  // 4x16 (output-)pixel patches per image
-  int kb_per_split;      // pixel patches per CTA (grid.z splits)
+  int total_kb;          // N * tiles_h * tiles_w
+  int n_co, n_ci, n_tiles;   // n_tiles = n_co * n_ci * taps
+  int chunks;            // pixel chunks: chunk c holds k-blocks [c * total_kb / chunks, (c + 1) * total_kb / chunks)
 };
 
-template <int BN, int T, int NPROD>
-struct WgradShape {
-  static constexpr int NSPLIT = NPROD == 3 ? 2 : 1;
-  static constexpr int A_STAGE = NSPLIT * TC_A_BYTES;         // 128 co x 64 px per plane
-  static constexpr int B_PLANE = BN * TC_BLOCK_K * 2;
-  static constexpr int B_STAGE = NSPLIT * B_PLANE;
-  static constexpr int SA = 2;
-  static constexpr int SB_RAW = (200 * 1024 - SA * A_STAGE) / B_STAGE;
-  static constexpr int SB = SB_RAW > 2 * T + 1 ? 2 * T + 1 : SB_RAW;   // the taps of two k-blocks in flight, one loading
-  static constexpr size_t SMEM = (size_t)SA * A_STAGE + (size_t)SB * B_STAGE + 1024;
-};
+struct WgradItem { int co0, ci0, tap, kb0, kb1; };
+__device__ __forceinline__ WgradItem wgrad_item(const TcWgradParams& p, int idx, int bn) {
+  const int c = idx / p.n_tiles;
+  int t = idx - c * p.n_tiles;
+  WgradItem it;
+  it.co0 = (t % p.n_co) * 128; t /= p.n_co;
+  it.ci0 = (t % p.n_ci) * bn;
+  it.tap = t / p.n_ci;
+  it.kb0 = (int)((int64_t)c * p.total_kb / p.chunks);
+  it.kb1 = (int)((int64_t)(c + 1) * p.total_kb / p.chunks);
+  return it;
+}
 
-template <int BN, int T, int NPROD>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+template <int BN, int NPROD>
+__global__ void __launch_bounds__(TC_WIDE_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_dy_hi, const __grid_constant__ CUtensorMap tm_dy_lo,
                 const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
                 const TcWgradParams p) {
-  using S = WgradShape<BN, T, NPROD>;
-  constexpr int NSPLIT = S::NSPLIT, A_STAGE = S::A_STAGE, B_PLANE = S::B_PLANE, B_STAGE = S::B_STAGE, SA = S::SA, SB = S::SB;
-  static_assert(SB >= 2 * T, "B ring too small");
-  static_assert(T * BN <= 192, "accumulators exceed the register budget");
-  constexpr int BOX_BYTES = 64 * 128;                          // one {64 c, 16 w, 4 h} box
+  constexpr int NSPLIT = NPROD == 3 ? 2 : 1;
+  constexpr int B_BYTES = BN * TC_BLOCK_K * 2;
+  constexpr int STAGE_BYTES = NSPLIT * (TC_A_BYTES + B_BYTES);
+  constexpr int STAGES = (192 * 1024) / STAGE_BYTES >= 8 ? 8 : (192 * 1024) / STAGE_BYTES;
+  static_assert(STAGES >= 2, "pipeline needs at least two stages");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + SA * A_STAGE;
-  __shared__ __align__(8) uint64_t full_a[SA], empty_a[SA], full_b[SB], empty_b[SB];
+  __shared__ __align__(8) uint64_t full_bar[STAGES];
+  __shared__ __align__(8) uint64_t empty_bar[STAGES];
+  __shared__ __align__(16) float s_stage[TC_CONSUMERS / 32][EPI_WARP_FLOATS];
 
   pdl_trigger();
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int ci_tiles = p.Cin / BN;
-  const int ci0 = (blockIdx.x % ci_tiles) * BN;
-  const int tap_row = blockIdx.x / ci_tiles;                   // filter row r (T == taps_w) or 0
-  const int co0 = blockIdx.y * 128;
-  const int total_kb = p.N * p.tiles_h * p.tiles_w;
-  const int kb_begin = blockIdx.z * p.kb_per_split;
-  const int kb_end = min(total_kb, kb_begin + p.kb_per_split);
-  const int num_kb = kb_end - kb_begin;
+  const int total_items = p.chunks * p.n_tiles;
   const int half = p.taps_w >> 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(&full_a[s]), 1); mbar_init(smem_u32(&empty_a[s]), TC_CONSUMERS / 32); }
-    for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(&full_b[s]), 1); mbar_init(smem_u32(&empty_b[s]), TC_CONSUMERS / 32); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), TC_CONSUMERS / 32); }
     fence_barrier_init();
     tma_prefetch_desc(&tm_dy_hi); tma_prefetch_desc(&tm_x_hi);
     if (NSPLIT == 2) { tma_prefetch_desc(&tm_dy_lo); tma_prefetch_desc(&tm_x_lo); }
   }
   __syncthreads();
   pdl_wait();
-  if (num_kb <= 0) return;
 
-  if (warp == TC_PRODUCER_WARP) {
-    if (lane == 0) {
-      for (int i = 0; i < num_kb; ++i) {
-        int kb = kb_begin + i;
-        const int tw = kb % p.tiles_w; kb /= p.tiles_w;
-        const int th = kb % p.tiles_h; const int n = kb / p.tiles_h;
-        const int h0 = th * 4, w0 = tw * 16;
-        const int sa = i % SA;
-        mbar_wait(smem_u32(&empty_a[sa]), ((i / SA) & 1) ^ 1);
-        const uint32_t bar_a = smem_u32(&full_a[sa]);
-        mbar_expect_tx(bar_a, A_STAGE);
+  if (warp >= TC_PRODUCER_WARP) {
+    // ===== TMA producer: 128 channels of dY + BN channels of X (shifted by the item's tap) per 64-pixel k-block
+    setmaxnreg_dec<40>();
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
+      uint32_t g = 0;                                  // global k-block counter across items -> ring slot / phase
+      for (int idx = blockIdx.x; idx < total_items; idx += gridDim.x) {
+        const WgradItem it = wgrad_item(p, idx, BN);
+        const int r = it.tap / p.taps_w, sx = it.tap - r * p.taps_w;
+        const int dh = (r - half) * p.dil, dw = (sx - half) * p.dil;
+        for (int kb = it.kb0; kb < it.kb1; ++kb, ++g) {
+          const int s = g % STAGES;
+          mbar_wait(smem_u32(&empty_bar[s]), ((g / STAGES) & 1) ^ 1);
+          const int tw = kb % p.tiles_w, q = kb / p.tiles_w;
+          const int th = q % p.tiles_h, n = q / p.tiles_h;
+          const int h0 = th * TC_SUB_H, w0 = tw * TC_SUB_W;
+          const int hh = h0 * p.stride + dh, ww = w0 * p.stride + dw;
+          uint8_t* stg = smem + (size_t)s * STAGE_BYTES;
+          const uint32_t bar = smem_u32(&full_bar[s]);
+          mbar_expect_tx(bar, STAGE_BYTES);
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {      // channels co0+64..127 of a 64-channel tensor are out of bounds = zeros
-          tma_load_4d(smem_u32(smem_a + sa * A_STAGE + hf * BOX_BYTES), &tm_dy_hi, bar_a, co0 + 64 * hf, w0, h0, n);
-          if (NSPLIT == 2)
-            tma_load_4d(smem_u32(smem_a + sa * A_STAGE + TC_A_BYTES + hf * BOX_BYTES), &tm_dy_lo, bar_a, co0 + 64 * hf, w0, h0, n);
-        }
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-          const int j = i * T + t;
-          const int sb = j % SB;
-          mbar_wait(smem_u32(&empty_b[sb]), ((j / SB) & 1) ^ 1);
-          const int r = (T == 1) ? half : tap_row;            // 1x1: the only tap; 3x3: this CTA's filter row
-          const int sx = (T == 1) ? half : t;
-          const int hh = h0 * p.stride + (r - half) * p.dil, ww = w0 * p.stride + (sx - half) * p.dil;
-          const uint32_t bar_b = smem_u32(&full_b[sb]);
-          mbar_expect_tx(bar_b, B_STAGE);
+          for (int hf = 0; hf < 2; ++hf) {      // channels co0+64..127 of a 64-channel tensor are out of bounds = zeros
+            tma_load_4d(smem_u32(stg + hf * TC_SUB_BYTES), &tm_dy_hi, bar, it.co0 + 64 * hf, w0, h0, n);
+            if (NSPLIT == 2) tma_load_4d(smem_u32(stg + TC_A_BYTES + hf * TC_SUB_BYTES), &tm_dy_lo, bar, it.co0 + 64 * hf, w0, h0, n);
+          }
 #pragma unroll
           for (int part = 0; part < BN / 64; ++part) {
-            tma_load_4d(smem_u32(smem_b + sb * B_STAGE + part * BOX_BYTES), &tm_x_hi, bar_b, ci0 + 64 * part, ww, hh, n);
+            tma_load_4d(smem_u32(stg + NSPLIT * TC_A_BYTES + part * TC_SUB_BYTES), &tm_x_hi, bar, it.ci0 + 64 * part, ww, hh, n);
             if (NSPLIT == 2)
-              tma_load_4d(smem_u32(smem_b + sb * B_STAGE + B_PLANE + part * BOX_BYTES), &tm_x_lo, bar_b, ci0 + 64 * part, ww, hh, n);
+              tma_load_4d(smem_u32(stg + 2 * TC_A_BYTES + B_BYTES + part * TC_SUB_BYTES), &tm_x_lo, bar, it.ci0 + 64 * part, ww, hh, n);
           }
         }
       }
     }
   } else {
+    // ===== consumer warpgroup wg: accumulator rows = output channels co0 + 64wg + 16w + lane/4 (+ 8), columns = input channels
+    setmaxnreg_inc<232>();
     const int wg = warp >> 2, w = warp & 3;
-    const bool live = co0 + 64 * wg < p.Cout;          // a 64-channel dY leaves the second warpgroup nothing to do
-    float acc[T][BN / 2];
-    for (int i = 0; i < num_kb; ++i) {
-      const int sa = i % SA;
-      mbar_wait(smem_u32(&full_a[sa]), (i / SA) & 1);
-      const uint32_t a_addr = smem_u32(smem_a + sa * A_STAGE + wg * BOX_BYTES);
-      const uint64_t a_hi = gmma_desc(a_addr, BOX_BYTES, 1024);
-      const uint64_t a_lo = gmma_desc(a_addr + TC_A_BYTES, BOX_BYTES, 1024);
-      wgmma_fence();
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        const int j = i * T + t;
-        const int sb = j % SB;
-        mbar_wait(smem_u32(&full_b[sb]), (j / SB) & 1);
-        const uint32_t b_addr = smem_u32(smem_b + sb * B_STAGE);
-        const uint64_t b_hi = gmma_desc(b_addr, BOX_BYTES, 1024);
-        const uint64_t b_lo = gmma_desc(b_addr + B_PLANE, BOX_BYTES, 1024);
-        if (live) {
-#pragma unroll
-          for (int k = 0; k < TC_BLOCK_K / 16; ++k) {
-            const uint64_t adv = (uint64_t)((k * 16 * 128) >> 4);     // 16 pixels = 16 rows of 128 bytes along K
-            mma_k16<BN, 1, NPROD>(acc[t], a_hi + adv, a_lo + adv, b_hi + adv, b_lo + adv, (i | k) != 0);
-          }
+    float* const st = s_stage[warp];
+    float acc[BN / 2], accx[BN / 2];
+    uint32_t g = 0;
+    for (int idx = blockIdx.x; idx < total_items; idx += gridDim.x) {
+      const WgradItem it = wgrad_item(p, idx, BN);
+      if (it.co0 + 64 * wg >= p.Cout) {               // a 64-channel dY leaves the second warpgroup nothing to do
+        for (int kb = it.kb0; kb < it.kb1; ++kb, ++g) {
+          mbar_wait(smem_u32(&full_bar[g % STAGES]), (g / STAGES) & 1);
+          if (lane == 0) mbar_arrive(smem_u32(&empty_bar[g % STAGES]));
         }
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                                  // k-block i - 1 is done: release its slots
-      if (i > 0 && lane == 0) {
-        mbar_arrive(smem_u32(&empty_a[(i - 1) % SA]));
+      } else {
+        conv_tc_mainloop<BN, BN, NPROD, STAGES, 1>(acc, accx, it.kb1 - it.kb0, g, full_bar, empty_bar, smem, wg, lane);
+        // lane l adds column 32c + l of the warp's 16 rows: 32 consecutive doubles per red instruction
+        double* const dst = p.dwp + ((size_t)it.tap * p.Cout + it.co0 + 64 * wg + 16 * w) * p.Cin + it.ci0 + lane;
 #pragma unroll
-        for (int t = 0; t < T; ++t) mbar_arrive(smem_u32(&empty_b[((i - 1) * T + t) % SB]));
-      }
-    }
-    wgmma_wait<0>();
+        for (int c = 0; c < BN / 32; ++c) {
+          stage_write(acc, c, st, lane);
 #pragma unroll
-    for (int t = 0; t < T; ++t) fence_acc(acc[t]);
-    if (live) {
-      const int co = co0 + 64 * wg + 16 * w + (lane >> 2);
-      const int ci = ci0 + 2 * (lane & 3);
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        const int tap = (T == 1) ? 0 : tap_row * p.taps_w + t;
-        double* dst = p.dwp + ((size_t)tap * p.Cout + co) * p.Cin + ci;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          red_add_f64(dst + 8 * j, (double)acc[t][4 * j]); red_add_f64(dst + 8 * j + 1, (double)acc[t][4 * j + 1]);
-          red_add_f64(dst + (size_t)8 * p.Cin + 8 * j, (double)acc[t][4 * j + 2]);
-          red_add_f64(dst + (size_t)8 * p.Cin + 8 * j + 1, (double)acc[t][4 * j + 3]);
+          for (int i = 0; i < 16; ++i) red_add_f64(dst + (size_t)i * p.Cin + 32 * c, (double)st[i * EPI_STRIDE + lane]);
+          __syncwarp();                                 // the tile is rewritten by the next chunk
         }
       }
     }
@@ -1419,19 +1398,37 @@ static bool tc_halo_enabled() {
   return v != 0;
 }
 
-template <int BN, int T, int NPROD>
+template <int BN, int NPROD>
 static int launch_wgrad_tc(const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi, const CUtensorMap& x_lo,
-                           const TcWgradParams& p, int splits, cudaStream_t st) {
-  const size_t smem = WgradShape<BN, T, NPROD>::SMEM;
+                           const TcWgradParams& p, int workers, cudaStream_t st) {
+  constexpr int NSPLIT = NPROD == 3 ? 2 : 1;
+  constexpr int STAGE_BYTES = NSPLIT * (TC_A_BYTES + BN * TC_BLOCK_K * 2);
+  constexpr int STAGES = (192 * 1024) / STAGE_BYTES >= 8 ? 8 : (192 * 1024) / STAGE_BYTES;
+  const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
   static bool configured = false;
   if (!configured) {
-    DDN_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, T, NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DDN_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int tap_rows = (T == 1) ? 1 : p.taps_w;
-  dim3 grid((unsigned)((p.Cin / BN) * tap_rows), (unsigned)ceil_div(p.Cout, 128), (unsigned)splits);
-  DDN_LAUNCH((wgrad_tc_kernel<BN, T, NPROD>), grid, TC_THREADS, smem, st, dy_hi, dy_lo, x_hi, x_lo, p);
+  DDN_LAUNCH((wgrad_tc_kernel<BN, NPROD>), workers, TC_WIDE_THREADS, smem, st, dy_hi, dy_lo, x_hi, x_lo, p);
   return 0;
+}
+
+// Pixel chunks of a weight gradient with `tiles` tiles over `total_kb` k-blocks on `workers` persistent CTAs: the smallest
+// count S whose round-robin makespan is within 2 % of an even split of the work, else the one with the smallest makespan.
+// The makespan is bounded by (items of the busiest CTA) x (longest chunk) = ceil(S * tiles / workers) * ceil(total_kb / S).
+// Fewer chunks mean fewer fp64 reds of partial tiles; chunks keep at least 4 k-blocks.
+static int tc_wgrad_chunks(int tiles, int total_kb, int workers) {
+  const double even = (double)tiles * total_kb / workers;
+  const int max_s = std::max(1, total_kb / 4);
+  int best = 1;
+  double best_span = 1e300;
+  for (int s = 1; s <= max_s; ++s) {
+    const double span = (double)ceil_div((int64_t)s * tiles, workers) * (double)ceil_div(total_kb, s);
+    if (span <= 1.02 * even) return s;
+    if (span < best_span) { best_span = span; best = s; }
+  }
+  return best;
 }
 
 // dwp[taps][Cout][Cin] += the weight gradient from the bf16 planes of x [N,H,W,Cin] and dy [N,Ho,Wo,Cout] (Ho = H/stride).
@@ -1473,8 +1470,7 @@ int tc_wgrad_planes(TcPlanes x, TcPlanes dy, float* dw, int N, int H, int W, int
     }
     return 0;
   }
-  // the T = 3 taps of a filter row keep 3 x BN accumulator columns in registers: BN = 64 there
-  const int bn = (k == 1 && Cin % 128 == 0) ? 128 : 64;
+  const int bn = Cin % 128 == 0 ? 128 : 64;
   CUtensorMap m_dy_hi, m_dy_lo, m_x_hi, m_x_lo;
   DDN_TRY(make_act_map(&m_dy_hi, dy.hi, N, Ho, Wo, Cout));
   DDN_TRY(make_act_map(&m_dy_lo, want_lo ? dy.lo : dy.hi, N, Ho, Wo, Cout));
@@ -1482,26 +1478,19 @@ int tc_wgrad_planes(TcPlanes x, TcPlanes dy, float* dw, int N, int H, int W, int
   DDN_TRY(make_act_map(&m_x_lo, want_lo ? x.lo : x.hi, N, H, W, Cin, stride));
   TcWgradParams p;
   p.dwp = dwp; p.N = N; p.H = Ho; p.W = Wo; p.Cin = Cin; p.Cout = Cout; p.taps_w = k; p.dil = dil; p.stride = stride;
-  p.tiles_h = (int)ceil_div(Ho, 4); p.tiles_w = (int)ceil_div(Wo, 16);
-  const int total_kb = N * p.tiles_h * p.tiles_w;
-  const int ctas_xy = (Cin / bn) * (k == 3 ? 3 : 1) * (int)ceil_div(Cout, 128);
-  // split-K so that the grid is (just under) a whole number of waves: 1 CTA per SM resident, no ragged tail wave
+  p.tiles_h = (int)ceil_div(Ho, TC_SUB_H); p.tiles_w = (int)ceil_div(Wo, TC_SUB_W);
+  p.total_kb = N * p.tiles_h * p.tiles_w;
+  p.n_co = (int)ceil_div(Cout, 128); p.n_ci = Cin / bn; p.n_tiles = p.n_co * p.n_ci * taps;
   const int sms = tc_worker_sms();
-  int waves = ctas_xy > sms ? 1 : (total_kb >= 64 * (sms / ctas_xy) ? 2 : 1);
-  int splits = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)waves * sms / ctas_xy, ceil_div(total_kb, 4)));
-  p.kb_per_split = (int)ceil_div(total_kb, splits);
-  splits = (int)ceil_div(total_kb, p.kb_per_split);
+  p.chunks = tc_wgrad_chunks(p.n_tiles, p.total_kb, sms);
+  const int workers = std::min(p.chunks * p.n_tiles, sms);
   const double fl = 2.0 * N * Ho * Wo * (double)Cout * taps * Cin;
   {
     ProfScope ps(PROF_CONV_WGRAD_TC, fl, st);
-#define WG(BNV, TV)                                                                                      \
-  do {                                                                                                   \
-    if (want_lo) DDN_TRY((launch_wgrad_tc<BNV, TV, 3>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, splits, st))); \
-    else DDN_TRY((launch_wgrad_tc<BNV, TV, 1>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, splits, st)));         \
-  } while (0)
-    if (k == 3) WG(64, 3);
-    else { if (bn == 128) WG(128, 1); else WG(64, 1); }
-#undef WG
+    if (bn == 128) DDN_TRY((want_lo ? launch_wgrad_tc<128, 3>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, workers, st)
+                                    : launch_wgrad_tc<128, 1>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, workers, st)));
+    else DDN_TRY((want_lo ? launch_wgrad_tc<64, 3>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, workers, st)
+                          : launch_wgrad_tc<64, 1>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, p, workers, st)));
   }
   if (dw) {
     int blocks = (int)std::min<int64_t>(ceil_div((int64_t)taps * Cout * Cin, 256), 4096);
