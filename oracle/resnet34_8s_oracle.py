@@ -151,6 +151,83 @@ def seeded_oracle(D=3, seed=0):
     return net
 
 
+STEM_PARAMS = ("resnet34_8s.conv1.weight", "resnet34_8s.bn1.weight", "resnet34_8s.bn1.bias")
+
+
+def decisive_biases(net, amp=6.0, on_fraction=0.7, seed=5):
+    """Sets every BatchNorm bias of the oracle ``net`` to +-amp (gammas stay 1) so that every ReLU input of the network lies
+    far from zero: the ReLU masks are then the same in every arithmetic and the whole-network gradient becomes a
+    well-conditioned function of the weights and inputs, which a tight per-tensor gate can test.
+
+    Each residual stage -- the stem plus layer1 (layer1.0's identity is the pooled stem output), layer2, layer3, layer4 --
+    draws ONE channel sign mask s (``on_fraction`` of the channels +1) and uses it for the stem bn1 (stage 0), every bn2 of
+    the stage and its downsample BatchNorm.  A channel that is on carries about +k*amp through the identity chain and one that
+    is off carries 0 (or -2*amp after a downsample), so no +amp meets a -amp at a residual add.  Each bn1 inside a block
+    draws its own mask.  What stays non-decisive is the stem's 3x3/2 max-pool (ties between window candidates), which only
+    reroutes gradient into STEM_PARAMS."""
+    r = net.resnet34_8s
+    g = torch.Generator().manual_seed(seed)
+
+    def mask(bn):
+        return (torch.rand(bn.num_features, generator=g) < on_fraction).to(bn.bias.dtype) * 2 - 1
+
+    with torch.no_grad():
+        for i, layer in enumerate((r.layer1, r.layer2, r.layer3, r.layer4)):
+            s = mask(layer[0].bn2)
+            if i == 0:
+                r.bn1.bias.copy_(amp * s)
+            for blk in layer:
+                blk.bn1.bias.copy_(amp * mask(blk.bn1))
+                blk.bn2.bias.copy_(amp * s)
+                if blk.downsample is not None:
+                    blk.downsample[1].bias.copy_(amp * s)
+    return net
+
+
+def rel(a, b):
+    """Relative Frobenius distance of a from b, in float64 on the host."""
+    a = a.detach().double().cpu(); b = b.detach().double().cpu()
+    return float((a - b).norm() / (b.norm() + 1e-30))
+
+
+def perturbed_relus(net, eps, seed):
+    """Multiplies every ReLU input of the oracle ``net`` by (1 + eps * N(0, 1)), elementwise, until the returned handles are
+    removed: the same network evaluated in an arithmetic whose forward error is ~eps.  Its gradient distance from the
+    unperturbed run measures how much the ReLU decisions that lie within ~eps of zero move each gradient tensor."""
+    gens = {}
+
+    def hook(_m, inp):
+        x = inp[0]
+        g = gens.setdefault(x.device, torch.Generator(device=x.device).manual_seed(seed))
+        return (x * (1 + eps * torch.randn(x.shape, generator=g, device=x.device, dtype=x.dtype)),)
+    return [m.register_forward_pre_hook(hook) for m in net.modules() if isinstance(m, nn.ReLU)]
+
+
+def gate_param_grads(got, g64, gate, label="", floor=None, floor_factor=4.0):
+    """got, g64: parameter name -> gradient; every tensor within `gate` of float64 (relative Frobenius norm).
+    - STEM_PARAMS sit behind the 3x3/2 max-pool, whose argmax cannot be made decisive (ONE window whose two best candidates
+      differ by less than the forward error reroutes one gradient element, ~1/sqrt(#windows) = 3e-3): gated at 2e-2.
+    - Tensors that vanish in float64 (fc.bias under the contrastive loss, where d/dA and d/dB cancel) stay negligible.
+    - floor: name -> distance of a float64 run with the forward perturbed at the product's error level (perturbed_relus).
+      Where a ReLU decision within that error of zero already moves a tensor beyond `gate`, the tensor is gated at
+      floor_factor times its floor instead: the product's own flips are a different draw of the same noise.
+    Returns the worst non-stem and the worst stem error."""
+    scale = max(float(v.double().norm()) for v in g64.values())
+    worst = worst_stem = 0.0
+    for k, r in g64.items():
+        if float(r.double().norm()) < 1e-6 * scale:
+            assert float(got[k].double().norm()) < 1e-4 * scale, "%s %s: should vanish" % (label, k)
+            continue
+        e = rel(got[k], r)
+        g = 2e-2 if k in STEM_PARAMS else max(gate, floor_factor * floor[k] if floor is not None else 0.0)
+        assert e < g, "%s %s: rel err %.3e (gate %.1e%s)" % (label, k, e, g, "" if floor is None else ", noise floor %.1e" % floor[k])
+        if k in STEM_PARAMS:
+            worst_stem = max(worst_stem, e)
+        else:
+            worst = max(worst, e)
+    return worst, worst_stem
+
+
 def process_network_output(image_pred, N, D, H, W):
     """dense_correspondence_network.py:303-319."""
     return image_pred.view(N, D, W * H).permute(0, 2, 1)

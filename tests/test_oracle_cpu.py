@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle import loss_oracle as LO
-from oracle.resnet34_8s_oracle import seeded_oracle, process_network_output
+from oracle.resnet34_8s_oracle import decisive_biases, seeded_oracle, process_network_output
 import pdc_b200
 from pdc_b200 import synthetic
 
@@ -119,6 +119,56 @@ def test_train_step_oracle_matches_golden(golden_dir):
         if k.startswith("grad:"):
             ref = g[k]; got = params[k[5:]].grad.numpy()
             assert np.linalg.norm(got - ref) <= 5e-3 * np.linalg.norm(ref) + 1e-7, k
+
+
+def _relu_input_margin(net, x):
+    """Smallest |ReLU input| over every ReLU call of a train-mode forward (the stem's, and both of every block: after bn1 and
+    after the residual add)."""
+    seen = []
+    hooks = [m.register_forward_pre_hook(lambda _m, inp: seen.append(float(inp[0].abs().min())))
+             for m in net.modules() if isinstance(m, torch.nn.ReLU)]
+    net.train()
+    with torch.no_grad():
+        net(x)
+    for h in hooks:
+        h.remove()
+    assert len(seen) == 1 + 2 * 16
+    return min(seen)
+
+
+def _independent_sign_biases(net, amp=3.0, on_fraction=0.7, seed=5):
+    """The construction decisive_biases replaced: an independent +-amp mask for every BatchNorm, so a -amp channel of bn2
+    can meet a positive identity at the residual add and their sum can land anywhere, zero included."""
+    g = torch.Generator().manual_seed(seed)
+    with torch.no_grad():
+        for k, p in net.named_parameters():
+            if ("bn" in k or "downsample.1" in k) and k.endswith(".bias"):
+                p.copy_(amp * ((torch.rand(p.shape, generator=g) < on_fraction).to(p.dtype) * 2 - 1))
+    return net
+
+
+def test_decisive_biases_keep_every_relu_input_away_from_zero():
+    """The construction behind the tight whole-network gradient gates (tests/test_gpu_network.py,
+    tests/test_gpu_training_size_gradients.py): in float64, at 64x96 with B = 2 and amp = 8, no ReLU input of the network
+    comes within MARGIN of zero, so a forward error of ~1e-5 (bf16x3) cannot flip a single ReLU decision.  The construction it
+    replaced fails the same check at its residual adds (smallest |input| ~1e-5).  MARGIN: the smallest |input| observed here
+    is 1.88 (layer1.2, after the residual add); 1.0 keeps a 2x cushion and is still ~10^4 times the forward error.  amp = 6
+    is not enough at this size (0.02): the zero-padded borders of the convolutions turn the constant offsets of the identity
+    chain into normalised outliers of up to |xhat| ~ 8."""
+    MARGIN, AMP = 1.0, 8.0
+    x = torch.randn(2, 3, 64, 96, generator=torch.Generator().manual_seed(77), dtype=torch.float64)
+    net = decisive_biases(seeded_oracle(D=3, seed=0).double(), amp=AMP)
+    for k, p in net.named_parameters():
+        if "bn" in k or "downsample.1" in k:
+            assert bool(torch.all(p == 1.0)) if k.endswith(".weight") else bool(torch.all(p.abs() == AMP)), k
+    assert _relu_input_margin(net, x) > MARGIN
+    # the inputs of tests/test_gpu_network.py::test_forward_pair_gradients_well_conditioned: each group normalised on its own,
+    # group B drawn with a shifted mean and a larger scale (smallest |input| observed: 1.93 for A, 1.87 for B)
+    gen = torch.Generator().manual_seed(78)
+    xa = torch.randn(2, 3, 64, 96, generator=gen); xb = 0.5 + 1.5 * torch.randn(2, 3, 64, 96, generator=gen)
+    assert _relu_input_margin(net, xa.double()) > MARGIN and _relu_input_margin(net, xb.double()) > MARGIN
+    old = _independent_sign_biases(seeded_oracle(D=3, seed=0).double(), amp=AMP)
+    assert _relu_input_margin(old, x) < MARGIN
 
 
 def test_synthetic_structure():
