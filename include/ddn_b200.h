@@ -259,6 +259,41 @@ int ddn_batchnorm_backward(const float* dy, const float* x, const float* y, cons
                            int64_t M, int C, int relu, void* workspace, size_t workspace_bytes, void* stream);
 size_t ddn_batchnorm_workspace_bytes(int64_t M, int C);
 
+/* Tensor-core convolutions with the fused epilogues the network runs (resnet.py:53-69 conv -> BatchNorm -> [+ residual] -> ReLU),
+ * one operator at a time.  precision BF16X3 or BF16 only (FP32_SIMT has no fused epilogues: DDN_EUNSUPPORTED), shapes as
+ * ddn_conv2d_forward's tensor-core path; every argument is checked before anything is launched.  bn_groups G (1 or 2, dividing N):
+ * images [g*N/G, (g+1)*N/G) form BatchNorm group g.  One workspace query serves all three. */
+size_t ddn_conv2d_fused_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil, int precision);
+/* Training forward: raw[N,Ho,Wo,Cout] = conv2d(x, w) and the batch statistics of raw per group, mean / invstd [G][Cout]
+ * (biased variance, invstd = 1/sqrt(var+eps)); running_mean / running_var [Cout] (both or neither) are updated group 0 first,
+ * then group 1, with `momentum` and the unbiased variance, like nn.BatchNorm2d in train().
+ * Cin = 3, k = 7, stride 2, pad 3 is the stem (resnet.py:127): x is then NCHW [N,3,H,W], the network's input layout, and the
+ * conv runs as the 7x7/2 patch GEMM. */
+int ddn_conv2d_bn_stats_forward(const float* x_nhwc, const float* w_oihw, float* raw_nhwc, float* mean, float* invstd,
+                                float* running_mean, float* running_var,
+                                int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil,
+                                int bn_groups, float momentum, float eps, int precision,
+                                void* workspace, size_t workspace_bytes, void* stream);
+/* Inference forward, eval-mode BatchNorm folded in: y = relu?(conv2d(x, w) * scale + shift + addend), scale = gamma /
+ * sqrt(running_var + eps), shift = beta - running_mean * scale; addend [N,Ho,Wo,Cout] fp32 may be NULL.  Outputs (at least one):
+ * fp32 y, and / or the bf16 operand planes y_hi = bf16(y), y_lo = bf16(y - y_hi) (y_lo written in BF16X3 only; may be NULL). */
+int ddn_conv2d_folded_forward(const float* x_nhwc, const float* w_oihw, const float* gamma, const float* beta,
+                              const float* running_mean, const float* running_var, const float* addend_nhwc,
+                              float* y_nhwc, void* y_hi_bf16, void* y_lo_bf16,
+                              int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil, int relu, float eps,
+                              int precision, void* workspace, size_t workspace_bytes, void* stream);
+/* Data gradient dx[N,H,W,Cin] = conv2d_input(dy[N,Ho,Wo,Cout], w) + addend (may be NULL), together with the column sums of the
+ * BatchNorm backward that consumes dx: that BatchNorm's output is y = relu(bn(raw) [+ residual]) with raw [N,H,W,Cin] and
+ * mean / invstd [G][Cin]; g = dx * (y > 0), the mask read from the bf16 hi plane of y (y_hi, blocks with a residual) or, when
+ * y_hi is NULL, recomputed from raw, gamma and beta.  sums [G][2][Cin] = (sum g, sum g * xhat) per group, dbeta = sum over
+ * groups of sum g, dgamma = of sum g * xhat. */
+int ddn_conv2d_backward_data_bn_stats(const float* w_oihw, const float* dy_nhwc, const float* addend_nhwc,
+                                      const float* raw_nhwc, const float* mean, const float* invstd, const float* gamma,
+                                      const float* beta, const void* y_hi_bf16,
+                                      float* dx_nhwc, float* dgamma, float* dbeta, float* sums,
+                                      int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil,
+                                      int bn_groups, int precision, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Bilinear align_corners=True resize of planar maps [N*C, h, w] -> [N*C, H, W]
  * (nn.functional.upsample_bilinear, resnet_dilated.py:320) and its adjoint. */
 int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, int h, int w, int H, int W, void* stream);

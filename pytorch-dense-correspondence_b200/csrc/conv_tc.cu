@@ -1776,8 +1776,8 @@ int tc_pack_all(const float* params, int64_t n_params, char* cache, const TcPack
 // staging layout: [weights hi|lo][x hi|lo][dy hi|lo][zero-inserted dy hi|lo (stride 2 only)]
 size_t tc_workspace_bytes(size_t max_act_elems) { return tc_weight_ws_bytes() + 6 * align_up(max_act_elems * 2, 1024) + 4096; }
 
-static int stage_planes(void* ws, size_t ws_bytes, size_t x_el, size_t dy_el, size_t up_el, void** wws, TcPlanes* x, TcPlanes* dy,
-                        TcPlanes* up) {
+int stage_planes(void* ws, size_t ws_bytes, size_t x_el, size_t dy_el, size_t up_el, void** wws, TcPlanes* x, TcPlanes* dy,
+                 TcPlanes* up) {
   char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
   const size_t wb = align_up(tc_weight_ws_bytes(), 1024), xb = align_up(x_el * 2, 1024), yb = align_up(dy_el * 2, 1024),
                ub = align_up(up_el * 2, 1024);

@@ -65,6 +65,8 @@ int tc_stem_forward(TcPlanes patches, const float* w_conv1, const TcPlanes* w_pa
 int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1, int W1, int precision, double* scratch, cudaStream_t st);
 
 // fp32-tensor wrappers (single-operator C ABI)
+// staging of those wrappers: weight packs, then the hi / lo planes of x, dy and the zero-inserted dy (x_el, dy_el, up_el elements)
+int stage_planes(void* ws, size_t ws_bytes, size_t x_el, size_t dy_el, size_t up_el, void** wws, TcPlanes* x, TcPlanes* dy, TcPlanes* up);
 int tc_conv_forward(const float* x_nhwc, const float* w_oihw, float* y_nhwc, int N, int H, int W, int Cin, int Cout,
                     int k, int stride, int pad, int dil, int precision, void* ws, size_t ws_bytes, cudaStream_t st);
 int tc_conv_backward(const float* x_nhwc, const float* w_oihw, const float* dy_nhwc, float* dx_nhwc, const float* dx_addend,

@@ -933,3 +933,121 @@ extern "C" int ddn_batchnorm_backward(const float* dy, const float* x, const flo
   a.M = M; a.C = C; a.relu = relu; a.training = 1; a.G = 1;
   return launch_bn_backward(a, st);
 }
+
+// ---- tensor-core convolutions with their fused epilogues (the variants the network's forward and backward run)
+// workspace: [BatchNorm accumulator + ticket][fold scale | shift][tensor-core staging (stage_planes)]
+static bool is_stem_shape(int Cin, int Cout, int k, int stride, int pad, int dil) {
+  return Cin == 3 && Cout == 64 && k == 7 && stride == 2 && pad == 3 && dil == 1;
+}
+static size_t fused_head_bytes(int C) { return bn_accum_bytes(C) + align_up(sizeof(float) * 2 * (size_t)C, 256); }
+
+extern "C" size_t ddn_conv2d_fused_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil,
+                                                   int precision) {
+  if (N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || precision == DDN_PRECISION_FP32_SIMT) return 0;
+  const int C = Cin > Cout ? Cin : Cout;
+  size_t act = (size_t)N * H * W * C;      // the stem stages its 7x7/2 patches instead of the NCHW input
+  if (is_stem_shape(Cin, Cout, k, stride, pad, dil)) act = (size_t)N * conv_out(H, 7, 2, 3, 1) * conv_out(W, 7, 2, 3, 1) * 192;
+  return fused_head_bytes(C) + tc_workspace_bytes(act) + 1024;
+}
+
+// every check of the fused entries, before anything is launched
+static int check_fused(int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil, int G, int precision,
+                       size_t ws_bytes, bool allow_stem) {
+  DDN_CHECK_ARG(precision >= DDN_PRECISION_FP32_SIMT && precision <= DDN_PRECISION_BF16, "unknown precision %d", precision);
+  if (precision == DDN_PRECISION_FP32_SIMT) {
+    set_error("the fused conv epilogues exist on the tensor-core path only (precision %d)", precision);
+    return DDN_EUNSUPPORTED;
+  }
+  DDN_CHECK_ARG(N >= 1 && H >= 8 && W >= 8, "bad sizes N=%d H=%d W=%d", N, H, W);
+  DDN_CHECK_ARG(G >= 1 && G <= BN_MAX_GROUPS && N % G == 0, "bn_groups must be 1 or %d and divide N (got %d for N=%d)", BN_MAX_GROUPS, G, N);
+  const bool stem = is_stem_shape(Cin, Cout, k, stride, pad, dil);
+  if (stem) {
+    if (!allow_stem) { set_error("the stem patch GEMM has no fused variant here"); return DDN_EUNSUPPORTED; }
+  } else if (!tc_conv_supported(Cin, Cout, k, stride, pad, dil, H, W)) {
+    set_error("shape not supported by the tensor-core path (Cin=%d Cout=%d k=%d stride=%d pad=%d dil=%d H=%d W=%d)", Cin, Cout, k, stride,
+              pad, dil, H, W);
+    return DDN_EUNSUPPORTED;
+  }
+  DDN_CHECK_ARG(ws_bytes >= ddn_conv2d_fused_workspace_bytes(N, H, W, Cin, Cout, k, stride, pad, dil, precision), "workspace too small");
+  return 0;
+}
+
+extern "C" int ddn_conv2d_bn_stats_forward(const float* x, const float* w, float* raw, float* mean, float* invstd, float* running_mean,
+                                           float* running_var, int N, int H, int W, int Cin, int Cout, int k, int stride, int pad,
+                                           int dil, int bn_groups, float momentum, float eps, int precision, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  DDN_CHECK_ARG(x && w && raw && mean && invstd && workspace, "null tensor");
+  DDN_CHECK_ARG(!running_mean == !running_var, "running_mean and running_var go together");
+  DDN_TRY(check_fused(N, H, W, Cin, Cout, k, stride, pad, dil, bn_groups, precision, workspace_bytes, true));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Ho = conv_out(H, k, stride, pad, dil), Wo = conv_out(W, k, stride, pad, dil);
+  const int C = Cin > Cout ? Cin : Cout;
+  char* ws = (char*)workspace;
+  BnFwdFinal fin;
+  fin.a = bn_accum_at(ws, C);
+  fin.mean = mean; fin.invstd = invstd; fin.running_mean = running_mean; fin.running_var = running_var;
+  fin.count = (int64_t)N / bn_groups * Ho * Wo; fin.G = bn_groups; fin.C = Cout; fin.momentum = momentum; fin.eps = eps;
+  DDN_CUDA(cudaMemsetAsync(ws, 0, bn_accum_bytes(C), st));
+  char* stage = ws + fused_head_bytes(C);
+  const size_t stage_bytes = workspace_bytes - fused_head_bytes(C);
+  void* wws; TcPlanes px, pdy, pup;
+  if (is_stem_shape(Cin, Cout, k, stride, pad, dil)) {      // x is NCHW [N,3,H,W]: 7x7/2 patch planes, then the K = 192 GEMM
+    DDN_TRY(stage_planes(stage, stage_bytes, (size_t)N * Ho * Wo * 192, 0, 0, &wws, &px, &pdy, &pup));
+    DDN_TRY(tc_stem_patches(x, const_cast<__nv_bfloat16*>(px.hi), const_cast<__nv_bfloat16*>(px.lo), N, H, W, precision, st));
+    return tc_stem_forward(px, w, nullptr, raw, &fin, N, Ho, Wo, precision, wws, tc_weight_ws_bytes(), st);
+  }
+  DDN_TRY(stage_planes(stage, stage_bytes, (size_t)N * H * W * Cin, 0, 0, &wws, &px, &pdy, &pup));
+  DDN_TRY(tc_split(x, const_cast<__nv_bfloat16*>(px.hi), const_cast<__nv_bfloat16*>(px.lo), (int64_t)N * H * W * Cin, precision, st));
+  return tc_conv_planes(px, w, nullptr, raw, nullptr, &fin, N, H, W, Cin, Cout, k, stride, dil, 0, precision, wws, tc_weight_ws_bytes(), st);
+}
+
+extern "C" int ddn_conv2d_folded_forward(const float* x, const float* w, const float* gamma, const float* beta, const float* running_mean,
+                                         const float* running_var, const float* addend, float* y, void* y_hi, void* y_lo,
+                                         int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil, int relu, float eps,
+                                         int precision, void* workspace, size_t workspace_bytes, void* stream) {
+  DDN_CHECK_ARG(x && w && gamma && beta && running_mean && running_var && workspace, "null tensor");
+  DDN_CHECK_ARG(y || y_hi, "the folded epilogue needs an output: y and / or the y_hi plane");
+  DDN_CHECK_ARG(y_hi || !y_lo, "y_lo is the low plane of y_hi");
+  DDN_TRY(check_fused(N, H, W, Cin, Cout, k, stride, pad, dil, 1, precision, workspace_bytes, false));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int C = Cin > Cout ? Cin : Cout;
+  char* ws = (char*)workspace;
+  float* scale = reinterpret_cast<float*>(ws + bn_accum_bytes(C)); float* shift = scale + Cout;
+  char* stage = ws + fused_head_bytes(C);
+  void* wws; TcPlanes px, pdy, pup;
+  DDN_TRY(stage_planes(stage, workspace_bytes - fused_head_bytes(C), (size_t)N * H * W * Cin, 0, 0, &wws, &px, &pdy, &pup));
+  DDN_TRY(launch_bn_fold(running_mean, running_var, gamma, beta, Cout, eps, scale, shift, st));
+  DDN_TRY(tc_split(x, const_cast<__nv_bfloat16*>(px.hi), const_cast<__nv_bfloat16*>(px.lo), (int64_t)N * H * W * Cin, precision, st));
+  TcFoldedEpilogue ep = {scale, shift, relu ? 1 : 0, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo};
+  return tc_conv_planes(px, w, nullptr, y, addend, nullptr, N, H, W, Cin, Cout, k, stride, dil, 0, precision, wws, tc_weight_ws_bytes(), st,
+                        &ep);
+}
+
+extern "C" int ddn_conv2d_backward_data_bn_stats(const float* w, const float* dy, const float* addend, const float* raw, const float* mean,
+                                                 const float* invstd, const float* gamma, const float* beta, const void* y_hi,
+                                                 float* dx, float* dgamma, float* dbeta, float* sums,
+                                                 int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil,
+                                                 int bn_groups, int precision, void* workspace, size_t workspace_bytes, void* stream) {
+  DDN_CHECK_ARG(w && dy && raw && mean && invstd && dx && dgamma && dbeta && sums && workspace, "null tensor");
+  DDN_CHECK_ARG(y_hi || (gamma && beta), "the recomputed ReLU mask (y_hi == NULL) needs gamma and beta");
+  DDN_TRY(check_fused(N, H, W, Cin, Cout, k, stride, pad, dil, bn_groups, precision, workspace_bytes, false));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Ho = conv_out(H, k, stride, pad, dil), Wo = conv_out(W, k, stride, pad, dil);
+  const int C = Cin > Cout ? Cin : Cout;
+  char* ws = (char*)workspace;
+  TcBwdStats bst;
+  memset(&bst, 0, sizeof(bst));
+  bst.raw = raw; bst.y_hi = (const __nv_bfloat16*)y_hi; bst.mean = mean; bst.invstd = invstd; bst.gamma = gamma; bst.beta = beta;
+  bst.relu = 1;
+  bst.fin.a = bn_accum_at(ws, C); bst.fin.sums = sums; bst.fin.dgamma = dgamma; bst.fin.dbeta = dbeta; bst.fin.G = bn_groups; bst.fin.C = Cin;
+  char* stage = ws + fused_head_bytes(C);
+  void* wws; TcPlanes px, pdy, pup;
+  DDN_TRY(stage_planes(stage, workspace_bytes - fused_head_bytes(C), 0, (size_t)N * Ho * Wo * Cout, stride == 2 ? (size_t)N * H * W * Cout : 0,
+                       &wws, &px, &pdy, &pup));
+  DDN_CUDA(cudaMemsetAsync(ws, 0, bn_accum_bytes(C), st));
+  if (stride == 2)      // zero insertion into the `up` planes, then a stride-1 data gradient
+    return tc_dgrad_strided(dy, pup, w, nullptr, dx, addend, N, H, W, Cin, Cout, k, precision, wws, tc_weight_ws_bytes(), st, &bst);
+  DDN_TRY(tc_split(dy, const_cast<__nv_bfloat16*>(pdy.hi), const_cast<__nv_bfloat16*>(pdy.lo), (int64_t)N * Ho * Wo * Cout, precision, st));
+  return tc_conv_planes(pdy, w, nullptr, dx, addend, nullptr, N, H, W, Cin, Cout, k, 1, dil, 1, precision, wws, tc_weight_ws_bytes(), st,
+                        nullptr, &bst);
+}

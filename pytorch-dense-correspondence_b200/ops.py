@@ -38,6 +38,79 @@ def conv2d_backward(x_nhwc, w_oihw, dy_nhwc, stride=1, pad=0, dil=1, need_dx=Tru
     return dx, dw
 
 
+def _out_hw(h, w, k, stride, pad, dil):
+    return (h + 2 * pad - dil * (k - 1) - 1) // stride + 1, (w + 2 * pad - dil * (k - 1) - 1) // stride + 1
+
+
+def _fused_ws(n, h, w, cin, cout, k, stride, pad, dil, precision, device):
+    nb = N.lib.ddn_conv2d_fused_workspace_bytes(n, h, w, cin, cout, k, stride, pad, dil, precision)
+    return _ws(nb, device)
+
+
+def conv2d_bn_stats_forward(x, w_oihw, stride=1, pad=0, dil=1, bn_groups=1, running_mean=None, running_var=None,
+                            momentum=0.1, eps=1e-5, precision=N.PRECISION_BF16X3):
+    """Tensor-core conv + the batch statistics of its output per BatchNorm group (training-forward epilogue).
+    x is NHWC, or NCHW [N,3,H,W] for the stem (Cin 3, 7x7, stride 2, pad 3).  running_mean / running_var are updated in place.
+    -> (raw [N,Ho,Wo,Cout], mean [G,Cout], invstd [G,Cout])"""
+    N.require_cuda_f32(x, "x"); N.require_cuda_f32(w_oihw, "w")
+    cout, cin, k, _ = w_oihw.shape
+    if cin == 3 and k == 7:
+        n, _, h, w = x.shape
+    else:
+        n, h, w, cin2 = x.shape
+        assert cin2 == cin
+    ho, wo = _out_hw(h, w, k, stride, pad, dil)
+    raw = torch.empty(n, ho, wo, cout, dtype=torch.float32, device=x.device)
+    mean = torch.empty(bn_groups, cout, dtype=torch.float32, device=x.device)
+    invstd = torch.empty_like(mean)
+    ws = _fused_ws(n, h, w, cin, cout, k, stride, pad, dil, precision, x.device)
+    N.check(N.lib.ddn_conv2d_bn_stats_forward(N.ptr(x), N.ptr(w_oihw), N.ptr(raw), N.ptr(mean), N.ptr(invstd), N.ptr(running_mean),
+                                              N.ptr(running_var), n, h, w, cin, cout, k, stride, pad, dil, bn_groups, momentum, eps,
+                                              precision, N.ptr(ws), ws.numel(), N.stream_ptr()))
+    return raw, mean, invstd
+
+
+def conv2d_folded_forward(x, w_oihw, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, addend=None, relu=True,
+                          eps=1e-5, want_y=True, want_planes=False, y_lo=None, precision=N.PRECISION_BF16X3):
+    """Tensor-core conv with eval-mode BatchNorm, addend and ReLU folded into its epilogue (inference).
+    want_planes: also (or, with want_y=False, only) the bf16 operand planes of y.  y_lo: optional caller tensor for the lo plane.
+    -> (y fp32 or None, y_hi bf16 or None, y_lo bf16 or None)"""
+    N.require_cuda_f32(x, "x"); N.require_cuda_f32(w_oihw, "w")
+    n, h, w, cin = x.shape
+    cout, _, k, _ = w_oihw.shape
+    ho, wo = _out_hw(h, w, k, stride, pad, dil)
+    y = torch.empty(n, ho, wo, cout, dtype=torch.float32, device=x.device) if want_y else None
+    y_hi = torch.empty(n, ho, wo, cout, dtype=torch.bfloat16, device=x.device) if want_planes else None
+    if want_planes and y_lo is None:
+        y_lo = torch.empty_like(y_hi)
+    ws = _fused_ws(n, h, w, cin, cout, k, stride, pad, dil, precision, x.device)
+    N.check(N.lib.ddn_conv2d_folded_forward(N.ptr(x), N.ptr(w_oihw), N.ptr(gamma), N.ptr(beta), N.ptr(running_mean), N.ptr(running_var),
+                                            N.ptr(addend), N.ptr(y), N.ptr(y_hi), N.ptr(y_lo), n, h, w, cin, cout, k, stride, pad, dil,
+                                            int(relu), eps, precision, N.ptr(ws), ws.numel(), N.stream_ptr()))
+    return y, y_hi, y_lo
+
+
+def conv2d_backward_data_bn_stats(w_oihw, dy, raw, mean, invstd, gamma, beta, stride=1, pad=0, dil=1, addend=None, y_hi=None,
+                                  precision=N.PRECISION_BF16X3):
+    """Tensor-core data gradient dx = conv2d_input(dy, w) + addend, with the column sums of the BatchNorm backward that consumes
+    dx (raw [N,H,W,Cin], mean / invstd [G,Cin]; ReLU mask from the bf16 plane y_hi, or recomputed from raw when y_hi is None).
+    -> (dx, dgamma [Cin], dbeta [Cin], sums [G,2,Cin])"""
+    N.require_cuda_f32(w_oihw, "w"); N.require_cuda_f32(dy, "dy"); N.require_cuda_f32(raw, "raw")
+    n, h, w, cin = raw.shape
+    cout, _, k, _ = w_oihw.shape
+    G = mean.shape[0]
+    dx = torch.empty_like(raw)
+    dgamma = torch.empty(cin, dtype=torch.float32, device=raw.device)
+    dbeta = torch.empty_like(dgamma)
+    sums = torch.empty(G, 2, cin, dtype=torch.float32, device=raw.device)
+    ws = _fused_ws(n, h, w, cin, cout, k, stride, pad, dil, precision, raw.device)
+    N.check(N.lib.ddn_conv2d_backward_data_bn_stats(N.ptr(w_oihw), N.ptr(dy), N.ptr(addend), N.ptr(raw), N.ptr(mean), N.ptr(invstd),
+                                                    N.ptr(gamma), N.ptr(beta), N.ptr(y_hi), N.ptr(dx), N.ptr(dgamma), N.ptr(dbeta),
+                                                    N.ptr(sums), n, h, w, cin, cout, k, stride, pad, dil, G, precision, N.ptr(ws),
+                                                    ws.numel(), N.stream_ptr()))
+    return dx, dgamma, dbeta, sums
+
+
 def batchnorm_forward(x, gamma, beta, residual=None, relu=False, training=True, running_mean=None, running_var=None,
                       momentum=0.1, eps=1e-5):
     """x [..., C] channels-last.  -> (y, save_mean, save_invstd)"""

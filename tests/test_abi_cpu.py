@@ -73,6 +73,42 @@ def test_workspace_and_argument_checks():
     assert N.lib.ddn_conv2d_workspace_bytes(1, 60, 80, 64, 64, 3, 1, 1, 1, 0) >= 3 * 9 * 64 * 64 * 4
     assert N.lib.ddn_batchnorm_workspace_bytes(4800, 6) == 0 and N.lib.ddn_batchnorm_workspace_bytes(4800, 512) > 0
     assert N.launch_count() == before
+    # the fused-epilogue conv entries: every refusal happens before the first launch (fake, never dereferenced pointers)
+    fake = ctypes.c_void_p(1 << 40)
+    big = 1 << 40
+    X3 = N.PRECISION_BF16X3
+    assert N.lib.ddn_conv2d_fused_workspace_bytes(2, 24, 32, 64, 64, 3, 1, 1, 1, X3) > 0
+    assert N.lib.ddn_conv2d_fused_workspace_bytes(2, 24, 32, 64, 64, 3, 1, 1, 1, N.PRECISION_FP32_SIMT) == 0
+
+    def stats(n=2, h=24, w=32, cin=64, cout=64, k=3, s=1, p=1, d=1, G=1, prec=X3, x=fake):
+        return N.lib.ddn_conv2d_bn_stats_forward(x, fake, fake, fake, fake, None, None, n, h, w, cin, cout, k, s, p, d, G, 0.1, 1e-5,
+                                                 prec, fake, big, None)
+
+    def folded(n=2, h=24, w=32, cin=64, cout=64, k=3, s=1, p=1, d=1, prec=X3, y=fake, y_hi=None, y_lo=None, x=fake):
+        return N.lib.ddn_conv2d_folded_forward(x, fake, fake, fake, fake, fake, None, y, y_hi, y_lo, n, h, w, cin, cout, k, s, p, d, 1,
+                                               1e-5, prec, fake, big, None)
+
+    def dgrad(n=2, h=24, w=32, cin=64, cout=64, k=3, s=1, p=1, d=1, G=1, prec=X3, dy=fake, y_hi=None, gamma=fake):
+        return N.lib.ddn_conv2d_backward_data_bn_stats(fake, dy, None, fake, fake, fake, gamma, fake, y_hi, fake, fake, fake, fake,
+                                                       n, h, w, cin, cout, k, s, p, d, G, prec, fake, big, None)
+
+    for call in (stats, dgrad):
+        assert call(G=3) == -1                                       # G = 3
+        assert call(n=3, G=2) == -1                                  # N % G != 0
+    assert stats(x=None) == -1 and folded(x=None) == -1 and dgrad(dy=None) == -1              # null pointers
+    assert folded(y=None) == -1                                      # no output at all
+    assert folded(y_lo=fake) == -1                                   # a lo plane without its hi plane
+    assert dgrad(gamma=None) == -1                                   # recomputed mask without gamma
+    for call in (stats, folded, dgrad):
+        assert call(prec=N.PRECISION_FP32_SIMT) == -3                # no fused epilogues on the CUDA cores
+        assert call(prec=7) == -1
+        assert call(cin=48) == -3                                    # unsupported shape
+        assert call(k=5, p=2) == -3
+    assert stats(n=3, h=64, w=96, cin=3, k=7, s=2, p=3, G=2) == -1  # stem: G does not divide N
+    assert folded(cin=3, k=7, s=2, p=3) == -3 and dgrad(cin=3, k=7, s=2, p=3) == -3
+    assert N.lib.ddn_conv2d_bn_stats_forward(fake, fake, fake, fake, fake, None, None, 2, 24, 32, 64, 64, 3, 1, 1, 1, 1, 0.1, 1e-5,
+                                             X3, fake, 1024, None) == -1             # workspace too small
+    assert N.launch_count() == before
     # SM reservation for a concurrent collective: a host-side setting with a range check (INTEGRATION.md A, data parallel)
     assert N.lib.ddn_set_reserved_sms(8) == 0 and N.lib.ddn_set_reserved_sms(0) == 0
     assert N.lib.ddn_set_reserved_sms(-1) == -1 and N.lib.ddn_set_reserved_sms(1000) == -1
