@@ -48,8 +48,6 @@ void set_error(const char* fmt, ...);
 // them (and, in the persistent tensor-core kernels, overlaps barrier initialisation with the predecessor's tail).
 // Rule: nothing written by an earlier kernel may be read before pdl_wait(), and EVERY thread of every kernel executes it
 // (a kernel that skipped it could finish before its predecessor and break the chain for its successor).
-// DDN_PDL=0 launches without the attribute (the instructions are then no-ops).
-bool pdl_enabled();
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -60,11 +58,9 @@ static inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 #endif

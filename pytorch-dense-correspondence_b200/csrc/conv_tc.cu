@@ -27,7 +27,6 @@
 // stride-1 1x1 downsample convs (resnet.py:210-214), plus their autograd data gradient.
 #include <cuda.h>
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <mutex>
@@ -240,6 +239,18 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
   return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
 
+// The fused epilogue request of conv_tc_kernel and conv64_halo_kernel (built and validated by tc_epilogue_request).
+struct TcEpilogueParams {
+  float* out;            // [N,H,W,C] fp32 (may be null with the folded epilogue)
+  const float* addend;   // optional, same shape
+  int imgs_per_group;    // BatchNorm group of image n = n / imgs_per_group
+  BnFwdFinal fin;        // fin.a.acc == nullptr: no statistics
+  TcBwdStats bst;        // bst.fin.a.acc != nullptr (data gradient): column sums of the BatchNorm backward that consumes `out`
+  // optional folded epilogue (inference): y = relu?(acc * ep_scale[c] + ep_shift[c] + addend)
+  const float* ep_scale; const float* ep_shift; int ep_relu;
+  __nv_bfloat16* out_hi; __nv_bfloat16* out_lo;
+};
+
 // The fused epilogue of a forward / data-gradient conv for EPI_ROWS pixels x 4 channels of one lane.  v[i] = accumulator of
 // pixel i; `off` = element offset of pixel 0, channel `ch` in the NHWC output (C channels per pixel), `rs` = elements between
 // pixel i and i + 1; only the first n_ok pixels exist (the others are neither stored nor summed).  Variants:
@@ -247,8 +258,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
 //   bst (data gradient): out = acc + addend, and (s1, s2) += (sum g, sum g * xhat), g = out * relu mask -- what
 //     bn_colsum_kernel<1> computes, on the gradient this kernel just wrote;
 //   otherwise (training forward): out = acc + addend, and (s1, s2) += the column sum / sum of squares of acc.
-template <typename P>
-__device__ __forceinline__ void conv_epilogue_rows(const P& p, const float4 (&v)[EPI_ROWS], size_t off, size_t rs, int n_ok, int ch,
+__device__ __forceinline__ void conv_epilogue_rows(const TcEpilogueParams& p, const float4 (&v)[EPI_ROWS], size_t off, size_t rs, int n_ok, int ch,
                                                    int C, int grp, float4& s1, float4& s2) {
   // the addend (residual-branch gradient) first: its global-load latency overlaps the rest
   float4 adv[EPI_ROWS];
@@ -340,6 +350,19 @@ __device__ __forceinline__ void colsum_lane_groups(float4& s1, float4& s2) {
 
 __device__ __forceinline__ void named_barrier(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
+// After a kernel's last item, in all TC_CONSUMERS consumer threads (named barrier `bar`): the CTA that arrives last turns the
+// accumulated sums of C channels into mean / invstd / running statistics (forward), or into dgamma / dbeta and the per-group
+// sums bn_bwd_apply_kernel reads (data gradient).
+__device__ __forceinline__ void conv_epilogue_finalize(const TcEpilogueParams& p, int C, int* s_last, int bar) {
+  if (p.fin.a.acc) {
+    if (bn_last_cta(p.fin.a.ticket, gridDim.x, threadIdx.x == 0, s_last, [bar] { named_barrier(bar, TC_CONSUMERS); }))
+      for (int c = threadIdx.x; c < C; c += TC_CONSUMERS) bn_fwd_finalize_channel(p.fin, c);
+  } else if (p.bst.fin.a.acc) {
+    if (bn_last_cta(p.bst.fin.a.ticket, gridDim.x, threadIdx.x == 0, s_last, [bar] { named_barrier(bar, TC_CONSUMERS); }))
+      for (int c = threadIdx.x; c < C; c += TC_CONSUMERS) bn_bwd_finalize_channel(p.bst.fin, c);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ the kernel
 // One persistent, warp-specialised kernel serves every convolution forward and data gradient: a 128-pixel x BLOCK_N tile per
 // work item, the two consumer warpgroups taking one 64-row sub-tile each.
@@ -356,8 +379,7 @@ __device__ __forceinline__ void named_barrier(int id, int threads) { asm volatil
 // accumulator (bn_stats.cuh), statistics finalized by the last CTA; inference -- eval-mode BN folded to
 // relu(acc*scale + shift + residual), written as fp32 and / or the next conv's bf16 planes; data gradient -- + addend.
 struct TcConvParams {
-  float* out;            // [N,H,W,Cout] fp32 (may be null with the folded epilogue)
-  const float* addend;   // optional, same shape
+  TcEpilogueParams epi;
   int N, H, W, Cin, Cout;   // H, W: OUTPUT size
   int taps_w;            // 1 or 3 (k x k filter)
   int dil;
@@ -366,12 +388,6 @@ struct TcConvParams {
   int n_sub;             // N * tiles_h * tiles_w
   int n_co;              // Cout / BLOCK_N
   int full_items, tail_split, total_items;
-  int imgs_per_group;    // BatchNorm group of image n = n / imgs_per_group
-  BnFwdFinal fin;        // fin.a.acc == nullptr: no statistics
-  TcBwdStats bst;        // bst.fin.a.acc != nullptr (data gradient): column sums of the BatchNorm backward that consumes `out`
-  // optional folded epilogue (inference): y = relu?(acc * ep_scale[c] + ep_shift[c] + addend)
-  const float* ep_scale; const float* ep_shift; int ep_relu;
-  __nv_bfloat16* out_hi; __nv_bfloat16* out_lo;
 };
 
 constexpr int TC_SUB_H = 4, TC_SUB_W = 16;     // sub-tile = one TMA box = 64 MMA rows
@@ -512,9 +528,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     setmaxnreg_inc<232>();
     const int wg = warp >> 2, w = warp & 3, e = threadIdx.x & 127;
     const int ga = lane >> 3, gb = lane & 7;
-    const bool stats = p.fin.a.acc != nullptr;
-    const bool bstats = p.bst.fin.a.acc != nullptr;
-    double* const sum_acc = bstats ? p.bst.fin.a.acc : p.fin.a.acc;
+    const bool stats = p.epi.fin.a.acc != nullptr;
+    const bool bstats = p.epi.bst.fin.a.acc != nullptr;
+    double* const sum_acc = bstats ? p.epi.bst.fin.a.acc : p.epi.fin.a.acc;
     float* const st = s_stage[warp];
     float acc[BLOCK_N / 2], accx[BLOCK_N / 2];
     uint32_t g = 0;
@@ -533,14 +549,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       const int n_ok = (sb.valid && h < p.H) ? min(EPI_ROWS, p.W - w4) : 0;          // valid pixels among the 4 (<= 0: none)
       const size_t pix = ((size_t)(n_ok > 0 ? sb.n : 0) * p.H + (n_ok > 0 ? h : 0)) * p.W + (n_ok > 0 ? w4 : 0);
       const size_t cbase = pix * p.Cout + it.co0 + gb * 4;                     // + i * Cout + c * 32
-      const int grp = sb.valid ? sb.n / p.imgs_per_group : 0;
+      const int grp = sb.valid ? sb.n / p.epi.imgs_per_group : 0;
 #pragma unroll
       for (int c = 0; c < BLOCK_N / 32; ++c) {
         if (c < (it.width >> 5)) {
           float4 v[EPI_ROWS];
           stage_chunk(acc, c, st, lane, v);
           float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;      // column sums of this lane's rows (4 channels)
-          conv_epilogue_rows(p, v, cbase + c * 32, (size_t)p.Cout, n_ok, it.co0 + c * 32 + gb * 4, p.Cout, grp, s1, s2);
+          conv_epilogue_rows(p.epi, v, cbase + c * 32, (size_t)p.Cout, n_ok, it.co0 + c * 32 + gb * 4, p.Cout, grp, s1, s2);
           if (stats || bstats) {
             colsum_lane_groups(s1, s2);
             if (ga == 0) {
@@ -563,15 +579,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         named_barrier(1 + wg, 128);          // s_part is rewritten by the next item
       }
     }
-    if (stats) {      // the last CTA turns the accumulated sums into mean / invstd / running statistics
-      const bool last = bn_last_cta(p.fin.a.ticket, gridDim.x, threadIdx.x == 0, &s_last, [] { named_barrier(3, TC_CONSUMERS); });
-      if (last)
-        for (int c = threadIdx.x; c < p.Cout; c += TC_CONSUMERS) bn_fwd_finalize_channel(p.fin, c);
-    } else if (bstats) {   // ... or into dgamma / dbeta and the per-group sums bn_bwd_apply_kernel reads
-      const bool last = bn_last_cta(p.bst.fin.a.ticket, gridDim.x, threadIdx.x == 0, &s_last, [] { named_barrier(3, TC_CONSUMERS); });
-      if (last)
-        for (int c = threadIdx.x; c < p.Cout; c += TC_CONSUMERS) bn_bwd_finalize_channel(p.bst.fin, c);
-    }
+    conv_epilogue_finalize(p.epi, p.Cout, &s_last, 3);
   }
 }
 
@@ -591,14 +599,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 // The plane ring has 3 slots in bf16 and 2 in bf16x3 (the resident lo weights take the room of the third); the halos of the
 // tiles two and three rounds ahead are pulled into L2 by prefetches that occupy no shared memory.
 struct TcHaloParams {
-  float* out; const float* addend;
+  TcEpilogueParams epi;
   int N, H, W;
   int tiles_h, tiles_w, n_tiles;
-  int imgs_per_group;
-  BnFwdFinal fin;
-  TcBwdStats bst;
-  const float* ep_scale; const float* ep_shift; int ep_relu;      // folded inference epilogue (see TcConvParams)
-  __nv_bfloat16* out_hi; __nv_bfloat16* out_lo;
 };
 constexpr int HALO_TH = 8, HALO_TW = 16;
 constexpr int HALO_BH = HALO_TH + 2, HALO_BW = HALO_TW + 2;
@@ -685,9 +688,9 @@ conv64_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
   } else {
     const int wg = warp >> 2, w = warp & 3;
     const int ga = lane >> 3, gb = lane & 7;
-    const bool stats = p.fin.a.acc != nullptr;
-    const bool bstats = p.bst.fin.a.acc != nullptr;     // data gradient: column sums of the BatchNorm backward that consumes `out`
-    double* const sum_acc = bstats ? p.bst.fin.a.acc : p.fin.a.acc;
+    const bool stats = p.epi.fin.a.acc != nullptr;
+    const bool bstats = p.epi.bst.fin.a.acc != nullptr;     // data gradient: column sums of the BatchNorm backward that consumes `out`
+    double* const sum_acc = bstats ? p.epi.bst.fin.a.acc : p.epi.fin.a.acc;
     float* const st = s_stage[warp];
     mbar_wait(smem_u32(&b_full), 0);
     const uint64_t bd_hi = gmma_desc_k(smem_u32(smem_b));
@@ -742,13 +745,13 @@ conv64_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
       // staging (the tiles are whole: H % 8 == 0, W % 16 == 0)
       const size_t pix0 = ((size_t)n * p.H + h0 + EPI_ROWS * (ga & 1)) * p.W + (w0 + 8 * wg + 2 * w + (ga >> 1));
       const size_t row_stride = (size_t)p.W * 64;      // floats between (h, w) and (h + 1, w)
-      const int grp = n / p.imgs_per_group;            // a tile lies inside one image
+      const int grp = n / p.epi.imgs_per_group;        // a tile lies inside one image
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         float4 v[EPI_ROWS];
         stage_chunk(acc, c, st, lane, v);
         float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;
-        conv_epilogue_rows(p, v, pix0 * 64 + gb * 4 + c * 32, row_stride, EPI_ROWS, c * 32 + gb * 4, 64, grp, s1, s2);
+        conv_epilogue_rows(p.epi, v, pix0 * 64 + gb * 4 + c * 32, row_stride, EPI_ROWS, c * 32 + gb * 4, 64, grp, s1, s2);
         if (stats || bstats) {
           colsum_lane_groups(s1, s2);
           if (ga == 0) {
@@ -769,15 +772,7 @@ conv64_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
         named_barrier(3, TC_CONSUMERS);                // s_part is rewritten by the next tile
       }
     }
-    if (bstats) {
-      const bool last = bn_last_cta(p.bst.fin.a.ticket, gridDim.x, threadIdx.x == 0, &s_last, [] { named_barrier(3, TC_CONSUMERS); });
-      if (last)
-        for (int c = threadIdx.x; c < 64; c += TC_CONSUMERS) bn_bwd_finalize_channel(p.bst.fin, c);
-    } else if (stats) {
-      const bool last = bn_last_cta(p.fin.a.ticket, gridDim.x, threadIdx.x == 0, &s_last, [] { named_barrier(3, TC_CONSUMERS); });
-      if (last)
-        for (int c = threadIdx.x; c < 64; c += TC_CONSUMERS) bn_fwd_finalize_channel(p.fin, c);
-    }
+    conv_epilogue_finalize(p.epi, 64, &s_last, 3);
   }
 }
 
@@ -1392,12 +1387,6 @@ static int make_weight_map(CUtensorMap* m, const void* base, int rows, int K, in
   return 0;
 }
 
-static bool tc_halo_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("DDN_TC_HALO"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v != 0;
-}
-
 template <int BN, int NPROD>
 static int launch_wgrad_tc(const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi, const CUtensorMap& x_lo,
                            const TcWgradParams& p, int workers, cudaStream_t st) {
@@ -1440,7 +1429,7 @@ int tc_wgrad_planes(TcPlanes x, TcPlanes dy, float* dw, int N, int H, int W, int
   const int taps = k * k;
   const int Ho = H / stride, Wo = W / stride;
   if (dw) DDN_TRY(launch_fill_zero(dwp, sizeof(double) * (size_t)taps * Cout * Cin, st));
-  if (tc_halo_enabled() && k == 3 && Cin == 64 && Cout == 64 && stride == 1 && dil == 1 && H % HALO_TH == 0 && W % HALO_TW == 0) {
+  if (k == 3 && Cin == 64 && Cout == 64 && stride == 1 && dil == 1 && H % HALO_TH == 0 && W % HALO_TW == 0) {
     // layer1: one halo tile of X + one tile of dY per 8x16 pixels, every tap read in place (wgrad64_halo_kernel)
     TcWgradHaloParams hp;
     hp.dwp = dwp; hp.N = N; hp.H = H; hp.W = W; hp.tiles_h = H / HALO_TH; hp.tiles_w = W / HALO_TW; hp.n_tiles = N * hp.tiles_h * hp.tiles_w;
@@ -1510,13 +1499,6 @@ int tc_unpack_wgrads(const TcUnpackEntry* entries, int n, const double* dwp_base
   return 0;
 }
 
-bool tc_available() { return true; }
-bool tc_folded_epilogue_supported() {      // DDN_FOLD_BN=0: keep the separate eval-mode BN pass (A/B measurements)
-  static int fold = -1;
-  if (fold < 0) { const char* e = getenv("DDN_FOLD_BN"); fold = (e && e[0] == '0') ? 0 : 1; }
-  return fold != 0;
-}
-
 // forward / weight-gradient coverage: 3x3 (pad == dil) or 1x1 (pad 0), stride 1 -- or stride 2 with dil 1 on even sizes
 bool tc_conv_supported(int Cin, int Cout, int k, int stride, int pad, int dil, int H, int W) {
   if (Cin % 64 || Cout % 64) return false;
@@ -1538,14 +1520,6 @@ int tc_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, in
   return 0;
 }
 
-int tc_pack_weights(const float* w_oihw, __nv_bfloat16* hi, __nv_bfloat16* lo, int Cout, int Cin, int k, int dgrad, int precision,
-                    cudaStream_t st) {
-  const size_t wel = (size_t)Cout * Cin * k * k;
-  int wblocks = (int)std::min<int64_t>(ceil_div((int64_t)wel, 256), 4096);
-  DDN_LAUNCH(pack_weights_tc_kernel, wblocks, 256, 0, st, w_oihw, hi, lo, Cout, Cin, k, dgrad, precision == DDN_PRECISION_BF16X3 ? 1 : 0);
-  return 0;
-}
-
 int tc_upsample_zero_split(const float* dy, __nv_bfloat16* hi, __nv_bfloat16* lo, int N, int Ho, int Wo, int C, int precision,
                            cudaStream_t st) {
   int64_t total = (int64_t)N * Ho * Wo * (C / 4);
@@ -1560,13 +1534,6 @@ int tc_stem_patches(const float* x_nchw, __nv_bfloat16* hi, __nv_bfloat16* lo, i
   dim3 grid((unsigned)ceil_div(W1, STEM_TW), (unsigned)H1, (unsigned)N);
   DDN_LAUNCH(stem_patch_split_kernel, grid, 256, 0, st, x_nchw, hi, lo, N, H, W, H1, W1, precision == DDN_PRECISION_BF16X3 ? 1 : 0);
   return 0;
-}
-
-// DDN_TC_TAIL=0: no N-split of the tail wave
-static bool tc_tail_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("DDN_TC_TAIL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v != 0;
 }
 
 template <int BLOCK_N, int NPROD>
@@ -1600,6 +1567,35 @@ static int launch_conv64_halo(const CUtensorMap& a_hi, const CUtensorMap& a_lo, 
   return 0;
 }
 
+// The epilogue request of one conv, for either kernel: `out` (+ `addend`) and at most one of the forward BatchNorm statistics
+// (`stats`), the data gradient's BatchNorm-backward column sums (`bst`) and the folded inference epilogue (`ep`).  A
+// BatchNorm request covers the gout channels the conv writes.
+static int tc_epilogue_request(TcEpilogueParams* e, float* out, const float* addend, const BnFwdFinal* stats, const TcBwdStats* bst,
+                               const TcFoldedEpilogue* ep, int N, int gout, int dgrad, int want_lo) {
+  memset(e, 0, sizeof(*e));
+  e->out = out; e->addend = addend; e->imgs_per_group = N;
+  if (stats) {
+    DDN_CHECK_ARG(!dgrad && !ep && stats->G >= 1 && stats->G <= BN_MAX_GROUPS && N % stats->G == 0 && stats->C == gout,
+                  "bad BatchNorm statistics request");
+    e->fin = *stats;
+    e->imgs_per_group = N / stats->G;
+  }
+  if (bst) {
+    DDN_CHECK_ARG(dgrad && !ep && !stats && bst->raw && bst->mean && bst->invstd && bst->fin.a.acc && bst->fin.G >= 1 &&
+                  bst->fin.G <= BN_MAX_GROUPS && N % bst->fin.G == 0 && bst->fin.C == gout && (bst->y_hi || !bst->relu || (bst->gamma && bst->beta)),
+                  "bad BatchNorm backward-statistics request");
+    e->bst = *bst;
+    e->imgs_per_group = N / bst->fin.G;
+  }
+  if (ep) {
+    DDN_CHECK_ARG(!dgrad && !stats && !bst && ep->scale && ep->shift && (out || ep->out_hi), "folded epilogue: forward only, needs scale/shift and an output");
+    e->ep_scale = ep->scale; e->ep_shift = ep->shift; e->ep_relu = ep->relu; e->out_hi = ep->out_hi; e->out_lo = want_lo ? ep->out_lo : nullptr;
+  } else {
+    DDN_CHECK_ARG(out != nullptr, "conv output pointer is null");
+  }
+  return 0;
+}
+
 // out[N,Ho,Wo,gout] = conv(planes of in[N,H,W,gin]) (+ addend).
 //   dgrad = 0: forward (gin = Cin, gout = Cout, Ho = H/stride).
 //   dgrad = 1: data gradient, stride 1 only (`in` = dY planes with Cout channels, out = dX with Cin channels; Cin/Cout are
@@ -1617,6 +1613,8 @@ int tc_conv_planes(TcPlanes in, const float* w_oihw, const TcPlanes* wpk, float*
   const double fl = 2.0 * N * Ho * Wo * (double)Cout * k * k * Cin;
   const int gin = dgrad ? Cout : Cin, gout = dgrad ? Cin : Cout;
   const int want_lo = precision == DDN_PRECISION_BF16X3;
+  TcEpilogueParams epi;
+  DDN_TRY(tc_epilogue_request(&epi, out, addend, stats, bst, ep, N, gout, dgrad, want_lo));
   const __nv_bfloat16* b_hi; const __nv_bfloat16* b_lo;
   if (wpk) {
     b_hi = wpk->hi; b_lo = wpk->lo;
@@ -1631,31 +1629,12 @@ int tc_conv_planes(TcPlanes in, const float* w_oihw, const TcPlanes* wpk, float*
     DDN_LAUNCH(pack_weights_tc_kernel, wblocks, 256, 0, st, w_oihw, ph, pl, Cout, Cin, k, dgrad, want_lo);
     b_hi = ph; b_lo = pl;
   }
-  if (tc_halo_enabled() && k == 3 && gin == 64 && gout == 64 && stride == 1 && dil == 1 && Ho % HALO_TH == 0 && Wo % HALO_TW == 0) {
+  if (k == 3 && gin == 64 && gout == 64 && stride == 1 && dil == 1 && Ho % HALO_TH == 0 && Wo % HALO_TW == 0) {
     // 64 -> 64 channels (layer1): resident weights + one halo tile per 8x16 output pixels (conv64_halo_kernel)
     TcHaloParams hp;
     memset(&hp, 0, sizeof(hp));
-    if (ep) {
-      DDN_CHECK_ARG(!dgrad && !stats && !bst && ep->scale && ep->shift && (out || ep->out_hi), "folded epilogue: forward only, needs scale/shift and an output");
-      hp.ep_scale = ep->scale; hp.ep_shift = ep->shift; hp.ep_relu = ep->relu; hp.out_hi = ep->out_hi; hp.out_lo = want_lo ? ep->out_lo : nullptr;
-    } else {
-      DDN_CHECK_ARG(out != nullptr, "conv output pointer is null");
-    }
-    hp.out = out; hp.addend = addend; hp.N = N; hp.H = Ho; hp.W = Wo;
+    hp.epi = epi; hp.N = N; hp.H = Ho; hp.W = Wo;
     hp.tiles_h = Ho / HALO_TH; hp.tiles_w = Wo / HALO_TW; hp.n_tiles = N * hp.tiles_h * hp.tiles_w;
-    hp.imgs_per_group = N;
-    if (stats) {
-      DDN_CHECK_ARG(!dgrad && stats->G >= 1 && stats->G <= BN_MAX_GROUPS && N % stats->G == 0 && stats->C == 64, "bad BatchNorm statistics request");
-      hp.fin = *stats;
-      hp.imgs_per_group = N / stats->G;
-    }
-    if (bst) {
-      DDN_CHECK_ARG(dgrad && !stats && bst->raw && bst->mean && bst->invstd && bst->fin.a.acc && bst->fin.G >= 1 && bst->fin.G <= BN_MAX_GROUPS &&
-                    N % bst->fin.G == 0 && bst->fin.C == 64 && (bst->y_hi || !bst->relu || (bst->gamma && bst->beta)),
-                    "bad BatchNorm backward-statistics request");
-      hp.bst = *bst;
-      hp.imgs_per_group = N / bst->fin.G;
-    }
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
     DDN_TRY(make_act_map_halo(&ma_hi, in.hi, N, H, W, 64));
     DDN_TRY(make_act_map_halo(&ma_lo, want_lo ? in.lo : in.hi, N, H, W, 64));
@@ -1667,7 +1646,7 @@ int tc_conv_planes(TcPlanes in, const float* w_oihw, const TcPlanes* wpk, float*
   const int block_n = gout % 128 == 0 ? 128 : 64;
   TcConvParams p;
   memset(&p, 0, sizeof(p));
-  p.out = out; p.addend = addend; p.N = N; p.H = Ho; p.W = Wo; p.Cin = gin; p.Cout = gout; p.taps_w = k; p.dil = dil;
+  p.epi = epi; p.N = N; p.H = Ho; p.W = Wo; p.Cin = gin; p.Cout = gout; p.taps_w = k; p.dil = dil;
   p.stride = stride;
   p.tiles_h = (int)ceil_div(Ho, TC_SUB_H); p.tiles_w = (int)ceil_div(Wo, TC_SUB_W);
   p.n_sub = N * p.tiles_h * p.tiles_w;
@@ -1677,30 +1656,11 @@ int tc_conv_planes(TcPlanes in, const float* w_oihw, const TcPlanes* wpk, float*
   // the tiles of the last, partial wave are cut along N so that the tail costs a fraction of a tile time
   const int rem = tiles % workers_max;
   int split = 1;
-  if (rem && tc_tail_enabled())
+  if (rem)
     while (split * 2 <= 8 && block_n / (split * 2) >= 32 && rem * split * 2 <= workers_max) split *= 2;
   p.full_items = tiles - rem; p.tail_split = split; p.total_items = p.full_items + rem * split;
   if (split == 1) { p.full_items = tiles; p.total_items = tiles; }
   const int workers = std::min(p.total_items, workers_max);
-  p.imgs_per_group = N;
-  if (stats) {
-    DDN_CHECK_ARG(!dgrad && !ep && stats->G >= 1 && stats->G <= BN_MAX_GROUPS && N % stats->G == 0, "bad BatchNorm statistics request");
-    p.fin = *stats;
-    p.imgs_per_group = N / stats->G;
-  }
-  if (bst) {
-    DDN_CHECK_ARG(dgrad && !ep && !stats && bst->raw && bst->mean && bst->invstd && bst->fin.a.acc && bst->fin.G >= 1 &&
-                  bst->fin.G <= BN_MAX_GROUPS && N % bst->fin.G == 0 && bst->fin.C == gout && (bst->y_hi || !bst->relu || (bst->gamma && bst->beta)),
-                  "bad BatchNorm backward-statistics request");
-    p.bst = *bst;
-    p.imgs_per_group = N / bst->fin.G;
-  }
-  if (ep) {
-    DDN_CHECK_ARG(!dgrad && !stats && ep->scale && ep->shift && (out || ep->out_hi), "folded epilogue: forward only, needs scale/shift and an output");
-    p.ep_scale = ep->scale; p.ep_shift = ep->shift; p.ep_relu = ep->relu; p.out_hi = ep->out_hi; p.out_lo = want_lo ? ep->out_lo : nullptr;
-  } else {
-    DDN_CHECK_ARG(out != nullptr, "conv output pointer is null");
-  }
   const int b_rows = block_n;
   const int bt_rows = b_rows / split;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo, mt_hi, mt_lo;

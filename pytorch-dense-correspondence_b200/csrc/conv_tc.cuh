@@ -11,7 +11,6 @@ struct TcPlanes { const __nv_bfloat16* hi; const __nv_bfloat16* lo; };   // x ~=
 // the conv (scale = gamma / sqrt(running_var + eps), shift = beta - running_mean * scale) -- written as fp32 (`out`, may be
 // null) and / or as the bf16 hi/lo operand planes of the next conv.
 struct TcFoldedEpilogue { const float* scale; const float* shift; int relu; __nv_bfloat16* out_hi; __nv_bfloat16* out_lo; };
-bool tc_folded_epilogue_supported();
 
 // Data-gradient epilogue that also produces the column sums of the BatchNorm backward consuming the gradient it writes:
 // out = dY of y = relu?(bn(raw) [+ residual]); g = out * (y > 0) with the mask taken from the bf16 hi plane of y (`y_hi`, blocks
@@ -25,7 +24,6 @@ struct TcBwdStats {
   BnBwdFinal fin;
 };
 
-bool tc_available();
 // forward / weight gradient: 3x3 (pad == dil) or 1x1 (pad 0), Cin and Cout multiples of 64, stride 1 (any dil) or 2 (dil 1)
 bool tc_conv_supported(int Cin, int Cout, int k, int stride, int pad, int dil, int H, int W);
 size_t tc_weight_ws_bytes();                       // staging for one conv's packed bf16 weights
@@ -38,8 +36,6 @@ int tc_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, in
 int tc_conv_planes(TcPlanes in, const float* w_oihw, const TcPlanes* w_packed, float* out, const float* addend, const BnFwdFinal* stats,
                    int N, int H, int W, int Cin, int Cout, int k, int stride, int dil, int dgrad, int precision,
                    void* wws, size_t wws_bytes, cudaStream_t st, const TcFoldedEpilogue* ep = nullptr, const TcBwdStats* bst = nullptr);
-int tc_pack_weights(const float* w_oihw, __nv_bfloat16* hi, __nv_bfloat16* lo, int Cout, int Cin, int k, int dgrad, int precision,
-                    cudaStream_t st);
 int tc_dgrad_strided(const float* dy_f32, TcPlanes up, const float* w_oihw, const TcPlanes* w_packed, float* dx, const float* addend,
                      int N, int H, int W, int Cin, int Cout, int k, int precision, void* wws, size_t wws_bytes, cudaStream_t st,
                      const TcBwdStats* bst = nullptr);

@@ -24,12 +24,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("DDN_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v != 0;
-}
-
 // SMs left free by the persistent tensor-core kernels (one CTA per SM, no room for a second): while a data-parallel host has a gradient
 // all-reduce in flight, NCCL's CTAs need somewhere to run -- without the reservation they take SMs between two of our launches and
 // the next persistent kernel runs a whole extra wave for the CTAs that found no SM.  Set by ddn_set_reserved_sms (DDN_RESERVED_SMS).
@@ -208,10 +202,6 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
   DDN_CHECK_ARG(D >= 1 && D <= 32, "descriptor dimension must be in [1,32] (got %d)", D);
   DDN_CHECK_ARG(precision >= DDN_PRECISION_FP32_SIMT && precision <= DDN_PRECISION_BF16, "unknown precision %d", precision);
   DDN_CHECK_ARG(mode >= DDN_MODE_INFER && mode <= DDN_MODE_EVAL_SAVE, "unknown mode %d", mode);
-  if (precision != DDN_PRECISION_FP32_SIMT && !tc_available()) {
-    set_error("precision %d needs the tensor-core conv path, which this build does not contain", precision);
-    return DDN_EUNSUPPORTED;
-  }
   const NetSpec& s = get_spec(D);
   p->B = B; p->H = H; p->W = W; p->D = D; p->mode = mode; p->precision = precision;
   const int G = BN_MAX_GROUPS;
@@ -255,6 +245,13 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
     if (b.has_ds) bb.ds = conv_bufs(b.ds, h, w);
     if (!p->tc) bb.out = f32((int64_t)B * bb.c2.Hout * bb.c2.Wout * b.c2.cout);
     bb.out_p = planes((int64_t)B * bb.c2.Hout * bb.c2.Wout * b.c2.cout);
+    // a tensor-core plan keeps no fp32 activations, so every block conv must have a tensor-core kernel (true for every H, W
+    // accepted above; a change of the spec or of that rule becomes an error here instead of a null read in a SIMT conv)
+    auto on_tc = [&](const ConvSpec& c, const ConvBufs& cb) { return tc_conv_supported(c.cin, c.cout, c.k, c.stride, c.pad, c.dil, cb.Hin, cb.Win); };
+    if (p->tc && !(on_tc(b.c1, bb.c1) && on_tc(b.c2, bb.c2) && (!b.has_ds || on_tc(b.ds, bb.ds)))) {
+      set_error("a block convolution at %dx%d has no tensor-core kernel (precision %d)", h, w, precision);
+      return DDN_EUNSUPPORTED;
+    }
     h = bb.c2.Hout; w = bb.c2.Wout;
     p->blk.push_back(bb);
   }
@@ -349,10 +346,6 @@ static const TcPlanes* cached_pack(const Ctx& c, const ConvSpec& cs, int dgrad, 
   return out;
 }
 
-static bool conv_on_tc(const Ctx& c, const ConvSpec& cs, int Hin, int Win) {
-  return c.p->tc && tc_conv_supported(cs.cin, cs.cout, cs.k, cs.stride, cs.pad, cs.dil, Hin, Win);
-}
-
 // BatchNorm statistics request of a forward conv: batch statistics accumulated by the conv epilogue (training), or none
 // (the statistics slots were filled from the running estimates by bn_eval_stats_all before the first conv)
 static BnFwdFinal stats_request(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, int64_t M) {
@@ -373,7 +366,7 @@ static int conv_bn_forward(const Ctx& c, const ConvSpec& cs, const BnSpec& bs, c
   float* raw = c.f(cb.raw);
   const int64_t M = (int64_t)N * cb.Hout * cb.Wout;
   const BnFwdFinal fin = stats_request(c, bs, cb, M);
-  if (conv_on_tc(c, cs, cb.Hin, cb.Win)) {
+  if (c.p->tc) {
     TcPlanes wpk_s; const TcPlanes* wpk = cached_pack(c, cs, 0, &wpk_s);
     return tc_conv_planes(c.planes(in_p), w, wpk, raw, nullptr, c.training() ? &fin : nullptr, N, cb.Hin, cb.Win, cs.cin, cs.cout, cs.k,
                           cs.stride, cs.dil, 0, c.p->precision, c.ws + c.p->wws, tc_weight_ws_bytes(), c.st);
@@ -424,7 +417,7 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   const NetSpec& s = *c.s; const Plan& p = *c.p;
   const int B = p.B, G = c.G;
   const bool want_lo = p.precision == DDN_PRECISION_BF16X3;
-  const bool fold = c.mode == DDN_MODE_INFER && p.tc && tc_folded_epilogue_supported();
+  const bool fold = c.mode == DDN_MODE_INFER && p.tc;
   DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(512), c.st));     // the workspace arrives uninitialised
   if (p.tc) DDN_TRY(ensure_packs(c));
   if (!c.training() && !fold) DDN_TRY(fill_eval_stats(c));
@@ -451,8 +444,7 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   for (size_t i = 0; i < s.blocks.size(); ++i) {        // BasicBlock.forward, resnet.py:53-69
     const BlockSpec& b = s.blocks[i]; const BlockBufs& bb = p.blk[i];
     int64_t M1 = (int64_t)B * bb.c1.Hout * bb.c1.Wout;
-    if (fold && conv_on_tc(c, b.c1, bb.c1.Hin, bb.c1.Win) && conv_on_tc(c, b.c2, bb.c2.Hin, bb.c2.Win) &&
-        (!b.has_ds || conv_on_tc(c, b.ds, bb.ds.Hin, bb.ds.Win))) {
+    if (fold) {
       DDN_TRY(conv_bn_folded(c, b.c1, b.b1, cur_p, bb.c1, B, nullptr, &bb.act1_p, nullptr, 1));       // act1: planes only
       // the epilogue's residual addend is fp32: the pooled stem output for the first block, else the previous block's fp32
       // output, which the folded path keeps in that block's (otherwise unused) c2.raw slot
@@ -513,7 +505,7 @@ static int conv_backward(const Ctx& c, const ConvSpec& cs, const float* in, cons
   const float* w = c.params + cs.w_off;
   float* dw = c.grads + cs.w_off;
   const double fl = 2.0 * N * Hout * Wout * (double)cs.cout * cs.k * cs.k * cs.cin;
-  if (conv_on_tc(c, cs, Hin, Win)) {
+  if (p.tc) {
     DDN_TRY(tc_wgrad_planes(c.planes(in_p), c.planes(p.grad_p), nullptr, N, Hin, Win, cs.cin, cs.cout, cs.k, cs.stride, cs.dil,
                             p.precision, c.d(p.dwp_all) + cs.w_off, c.st));
     if (dx) {
@@ -551,7 +543,7 @@ static int conv_backward(const Ctx& c, const ConvSpec& cs, const float* in, cons
 // fp32 for a SIMT conv.  mask: the bf16 hi plane of y / the fp32 y / recomputed from raw (no residual) -- see BnBwdArgs.
 // fused_slot > 0: the column sums were produced by the data-gradient epilogue that wrote `dy` (bwd_stats_for) -- skip that pass.
 static int bn_backward_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, const float* dy, const float* y_f32,
-                           const __nv_bfloat16* y_hi, int relu, float* g_out, const ConvSpec& cs, int Hin, int Win, float* dx_f32, int64_t M,
+                           const __nv_bfloat16* y_hi, int relu, float* g_out, const ConvSpec& cs, float* dx_f32, int64_t M,
                            int fused_slot = 0) {
   BnBwdArgs a;
   memset(&a, 0, sizeof(a));
@@ -562,7 +554,7 @@ static int bn_backward_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, c
   a.acc = c.accum(); a.sums = c.f(c.p->sums) + (size_t)fused_slot * 2 * c.G * 512;
   a.sums_ready = fused_slot > 0;
   a.M = M; a.C = bs.C; a.relu = relu; a.training = c.training() ? 1 : 0; a.G = c.G;
-  if (conv_on_tc(c, cs, Hin, Win)) {
+  if (c.p->tc) {
     a.dx = cs.stride == 2 ? dx_f32 : nullptr;      // the strided data gradient re-reads dY in fp32 (zero insertion)
     a.dx_hi = c.h(c.p->grad_p.hi);
     a.dx_lo = c.p->precision == DDN_PRECISION_BF16X3 ? c.h(c.p->grad_p.lo) : nullptr;
@@ -573,15 +565,9 @@ static int bn_backward_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, c
 }
 
 // Column sums of BatchNorm `bs` (y = relu(bn(raw) [+ residual])) computed by the epilogue of the tensor-core data gradient that
-// produces its dY (conv_tc.cuh TcBwdStats) instead of a separate pass over dY and raw.  DDN_FUSE_BWD_STATS_MINC (default 64 = every
-// layer) keeps the separate pass for layers narrower than that many channels (A/B switch).
-static int fuse_bwd_stats_min_c() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("DDN_FUSE_BWD_STATS_MINC"); v = e ? atoi(e) : 64; if (v < 0) v = 0; }
-  return v;
-}
+// produces its dY (conv_tc.cuh TcBwdStats) instead of a separate pass over dY and raw.
 static bool bwd_stats_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, const __nv_bfloat16* y_hi, int slot, TcBwdStats* out) {
-  if (!c.p->tc || bs.C < fuse_bwd_stats_min_c()) return false;
+  if (!c.p->tc) return false;
   memset(out, 0, sizeof(*out));
   out->raw = c.f(cb.raw); out->y_hi = y_hi; out->mean = c.mean(cb.stats); out->invstd = c.invstd(cb.stats, bs.C);
   out->gamma = c.params + bs.g_off; out->beta = c.params + bs.b_off; out->relu = 1;
@@ -609,8 +595,8 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
                              (p.tc && want_lo) ? c.h(last.out_p.lo) : nullptr, c.params + s.fc_w, S[cur], c.grads + s.fc_w,
                              c.grads + s.fc_b, c.f(p.fc_part), (int64_t)h8 * w8, B, 512, p.D, c.st));
   std::vector<TcUnpackEntry> pending;      // tensor-core weight gradients waiting in dwp_all for the bucket's conversion
-  auto defer = [&](const ConvSpec& cs, int Hin, int Win) {
-    if (!conv_on_tc(c, cs, Hin, Win)) return;
+  auto defer = [&](const ConvSpec& cs) {
+    if (!p.tc) return;
     TcUnpackEntry e; e.src_off = cs.w_off; e.dst_off = cs.w_off; e.Cout = cs.cout; e.Cin = cs.cin; e.taps = cs.k * cs.k; e.kind = 0;
     pending.push_back(e);
   };
@@ -636,37 +622,36 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
     int t1 = (cur + 1) & 3, t2 = (cur + 2) & 3, t3 = (cur + 3) & 3;
     // out = relu(bn2(raw2) + residual):  g = dOut*(out>0) -> S[t2];  d raw2 -> planes (tensor core) or S[t1] (fp32)
     DDN_TRY(bn_backward_for(c, b.b2, bb.c2, S[cur], p.tc ? nullptr : c.f(bb.out), p.tc ? c.h(bb.out_p.hi) : nullptr, 1, S[t2], b.c2,
-                            bb.c2.Hin, bb.c2.Win, S[t1], M1, b2_fused ? 2 : 0));
+                            S[t1], M1, b2_fused ? 2 : 0));
     // conv2: dW, d act1 -> S[t3] (+ the column sums of bn1's backward, in the same epilogue)
     TcBwdStats st1, st2;
-    const bool b1_fused = conv_on_tc(c, b.c2, bb.c2.Hin, bb.c2.Win) && bwd_stats_for(c, b.b1, bb.c1, nullptr, 1, &st1);
+    const bool b1_fused = bwd_stats_for(c, b.b1, bb.c1, nullptr, 1, &st1);
     DDN_TRY(conv_backward(c, b.c2, p.tc ? nullptr : c.f(bb.act1), bb.act1_p, S[t1], S[t3], nullptr, B, bb.c2.Hin, bb.c2.Win, bb.c2.Hout,
                           bb.c2.Wout, b.c2.cin, b1_fused ? &st1 : nullptr));
-    defer(b.c2, bb.c2.Hin, bb.c2.Win);
+    defer(b.c2);
     // conv1's data gradient completes d(block input) = dOut of the previous block: bn2 of that block gets its column sums there
-    b2_fused = i > 0 && conv_on_tc(c, b.c1, bb.c1.Hin, bb.c1.Win) &&
-               bwd_stats_for(c, s.blocks[i - 1].b2, p.blk[i - 1].c2, c.h(p.blk[i - 1].out_p.hi), 2, &st2);
+    b2_fused = i > 0 && bwd_stats_for(c, s.blocks[i - 1].b2, p.blk[i - 1].c2, c.h(p.blk[i - 1].out_p.hi), 2, &st2);
     // act1 = relu(bn1(raw1)), no residual: the mask is recomputed from raw1 in the tensor-core modes
     if (!b.has_ds) {
-      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, bb.c1.Hin, bb.c1.Win, S[t1], M1,
+      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, S[t1], M1,
                               b1_fused ? 1 : 0));
       // dX = dgrad(conv1) + g
       DDN_TRY(conv_backward(c, b.c1, xin, xin_p, S[t1], S[t3], S[t2], B, bb.c1.Hin, bb.c1.Win, bb.c1.Hout, bb.c1.Wout, b.c1.cin,
                             b2_fused ? &st2 : nullptr));
-      defer(b.c1, bb.c1.Hin, bb.c1.Win);
+      defer(b.c1);
       cur = t3;
     } else {
       // residual branch first (its dY planes are consumed before conv1's overwrite them):
       // bn_d(raw_d): d raw_d; ds conv: dW, dX_ds -> S[cur]
-      DDN_TRY(bn_backward_for(c, b.bd, bb.ds, S[t2], nullptr, nullptr, 0, nullptr, b.ds, bb.ds.Hin, bb.ds.Win, S[t1], M1));
+      DDN_TRY(bn_backward_for(c, b.bd, bb.ds, S[t2], nullptr, nullptr, 0, nullptr, b.ds, S[t1], M1));
       DDN_TRY(conv_backward(c, b.ds, xin, xin_p, S[t1], S[cur], nullptr, B, bb.ds.Hin, bb.ds.Win, bb.ds.Hout, bb.ds.Wout, b.ds.cin));
-      defer(b.ds, bb.ds.Hin, bb.ds.Win);
+      defer(b.ds);
       // main branch: d raw1, then dX = dgrad(conv1) + dX_ds -> S[t2]
-      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, bb.c1.Hin, bb.c1.Win, S[t1], M1,
+      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, S[t1], M1,
                               b1_fused ? 1 : 0));
       DDN_TRY(conv_backward(c, b.c1, xin, xin_p, S[t1], S[t2], S[cur], B, bb.c1.Hin, bb.c1.Win, bb.c1.Hout, bb.c1.Wout, b.c1.cin,
                             b2_fused ? &st2 : nullptr));
-      defer(b.c1, bb.c1.Hin, bb.c1.Win);
+      defer(b.c1);
       cur = t2;
       // a block with a downsample branch opens a residual layer: everything from its first parameter up is final now
       DDN_TRY(close_bucket(b.c1.w_off));     // layer4 (+fc), layer3, layer2; layer1 + stem close at the end

@@ -15,7 +15,6 @@
 // the channel-strided NCHW gather) to the 16 bytes of the two indices.
 //
 // Descriptor images: low_a / low_b [B, h*w, D] fp32 (what ddn_resnet34_8s_forward writes to `low_nhwc_out`).
-#include <cstdlib>
 #include "bn_stats.cuh"
 #include "loss.cuh"
 
@@ -268,7 +267,8 @@ __device__ __forceinline__ float4 quad_diff(const float* __restrict__ A, const f
 
 // LR_FWD_ITEMS index pairs per lane group in the forward: that many times fewer blocks = fewer contended atomics on the
 // B * n_terms accumulators (they bound the one-pair version), and 8 * LR_FWD_ITEMS loads in flight per lane
-template <int LPP, int LR_FWD_ITEMS>
+constexpr int LR_FWD_ITEMS = 4;
+template <int LPP>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_fwd_quad_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, float sh, float sw,
                             const __grid_constant__ DevTerms T, double* __restrict__ sums, unsigned long long* __restrict__ counts) {
@@ -456,10 +456,8 @@ extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const fl
   DDN_TRY(check_common(low_a, low_b, B, (int64_t)H * W, D, W));
   DDN_CHECK_ARG(sums && counts && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null outputs");
   const int lpp = (D == 8 || D == 16 || D == 32) ? D / 4 : 1;
-  // 4 pairs per lane group; 8 (DDN_LOSS_FWD_ITEMS=8) halves the atomics again but costs occupancy
-  static const int items = [] { const char* e = getenv("DDN_LOSS_FWD_ITEMS"); return (e && atoi(e) == 8) ? 8 : 4; }();
   DevTerms T;
-  DDN_TRY(build_terms_lr(terms_host, n_terms, &T, lpp > 1 ? LR_THREADS / lpp * items : LR_THREADS));
+  DDN_TRY(build_terms_lr(terms_host, n_terms, &T, lpp > 1 ? LR_THREADS / lpp * LR_FWD_ITEMS : LR_THREADS));
   cudaStream_t st = (cudaStream_t)stream;
   DDN_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * B * n_terms, st));
   DDN_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * B * n_terms, st));
@@ -471,11 +469,7 @@ extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const fl
   ProfScope ps(PROF_LOSS_FWD, pairs * (16.0 + 8.0 * D), st);
   const float sh = ac_scale(h, H), sw = ac_scale(w, W);
 #define FWD(DT) DDN_LAUNCH(loss_lowres_fwd_kernel<DT>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, sums, cnt)
-#define FWDQ(L)                                                                                                                              \
-  do {                                                                                                                                       \
-    if (items == 4) DDN_LAUNCH((loss_lowres_fwd_quad_kernel<L, 4>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt); \
-    else DDN_LAUNCH((loss_lowres_fwd_quad_kernel<L, 8>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt);            \
-  } while (0)
+#define FWDQ(L) DDN_LAUNCH(loss_lowres_fwd_quad_kernel<L>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt)
   switch (D) {
     case 3: FWD(3); break;
     case 4: FWD(4); break;
