@@ -127,6 +127,36 @@ size_t ddn_resnet34_8s_weight_cache_bytes(int D);
 int ddn_resnet34_8s_set_weight_cache(void* cache, size_t bytes, const float* params, uint64_t version, int precision);
 
 /* ------------------------------------------------------------------------------------------
+ * The same entry points for a backbone chosen by id, as the reference picks it by name
+ * (dense_correspondence/network/dense_correspondence_network.py:360-383):
+ *   DDN_ARCH_RESNET34_8S  Resnet34_8s, BasicBlock [3, 4, 6, 3]   (the ddn_resnet34_8s_* functions above)
+ *   DDN_ARCH_RESNET50_8S  Resnet50_8s, Bottleneck [3, 4, 6, 3], 2048-channel trunk, fc = Conv2d(2048, D, 1)
+ *                         (PSD/pytorch_segmentation_detection/models/resnet_dilated.py:399-435, resnet.py:72-109)
+ * Arguments and results are those of the ddn_resnet34_8s_* function of the same suffix; table names are the state-dict keys
+ * without the leading "resnet50_8s." (320 entries: 161 learnable tensors, 106 running statistics, 53 num_batches_tracked).
+ * An unknown arch returns DDN_EINVAL (0 from the size queries).  ddn_resnet34_8s_set_weight_cache serves every architecture.
+ * ------------------------------------------------------------------------------------------ */
+enum { DDN_ARCH_RESNET34_8S = 0, DDN_ARCH_RESNET50_8S = 1 };
+
+int ddn_net_param_table(int arch, int D, ddn_tensor_entry* out, int cap);
+int ddn_net_buffer_table(int arch, ddn_tensor_entry* out, int cap);
+int64_t ddn_net_param_count(int arch, int D);
+int64_t ddn_net_buffer_count(int arch);
+size_t ddn_net_workspace_bytes(int arch, int B, int H, int W, int D, int mode, int precision);
+int ddn_net_forward(int arch, const float* x, const float* params, float* buffers, float* y,
+                    void* workspace, size_t workspace_bytes,
+                    int B, int H, int W, int D,
+                    int mode, int bn_groups, float momentum, float eps, int precision,
+                    float* low_nhwc_out, void* stream);
+int ddn_net_backward(int arch, const float* dy, const float* dlow_nhwc, const float* params, float* grads,
+                     void* workspace, size_t workspace_bytes,
+                     int B, int H, int W, int D, int mode, int bn_groups, float eps, int precision,
+                     ddn_grad_bucket_fn on_bucket, void* user, void* stream);
+/* 4 buckets for both architectures: layer4 + fc, layer3, layer2, layer1 + stem. */
+int ddn_net_grad_buckets(int arch, int D, int64_t* offsets, int cap);
+size_t ddn_net_weight_cache_bytes(int arch, int D);
+
+/* ------------------------------------------------------------------------------------------
  * Pixelwise contrastive loss.
  * Descriptor images are addressed with explicit strides so the reference's strided view
  *   process_network_output: [N,D,H,W].view(N,D,W*H).permute(0,2,1)

@@ -7,7 +7,7 @@ Everything numerical happens in ``libddn_b200.so`` (C ABI in include/ddn_b200.h)
 raises if that library is missing -- there is no CPU / PyTorch fallback.
 """
 from . import _native
-from .resnet_dilated import Resnet34_8s, set_default_precision
+from .resnet_dilated import Resnet34_8s, Resnet50_8s, set_default_precision
 from .dense_correspondence_network import DenseCorrespondenceNetwork
 from .pixelwise_contrastive_loss import PixelwiseContrastiveLoss, DEFAULT_LOSS_CONFIG
 from . import loss_composer
@@ -15,5 +15,5 @@ from .loss_composer import SpartanDatasetDataType
 from .fused_adam import FusedAdam, adjust_learning_rate
 from . import ops, synthetic, data_parallel, sampling
 
-__all__ = ["Resnet34_8s", "DenseCorrespondenceNetwork", "PixelwiseContrastiveLoss", "loss_composer",
+__all__ = ["Resnet34_8s", "Resnet50_8s", "DenseCorrespondenceNetwork", "PixelwiseContrastiveLoss", "loss_composer",
            "SpartanDatasetDataType", "DEFAULT_LOSS_CONFIG", "set_default_precision", "FusedAdam", "adjust_learning_rate", "ops", "synthetic", "data_parallel", "sampling"]

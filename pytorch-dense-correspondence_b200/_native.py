@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libddn_b200.so")
 
 PRECISION_FP32_SIMT, PRECISION_BF16X3, PRECISION_BF16 = 0, 1, 2
 MODE_INFER, MODE_TRAIN, MODE_EVAL_SAVE = 0, 1, 2
+ARCH_RESNET34_8S, ARCH_RESNET50_8S = 0, 1
 GRAD_BUCKET_FN = ctypes.CFUNCTYPE(None, ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int64)
 TERM_MATCH, TERM_HINGE, TERM_HINGE_INV = 0, 1, 2
 TERM_PIXEL_WEIGHT = 1
@@ -61,6 +62,15 @@ _SIGNATURES = {
     "ddn_contrastive_terms_backward_lowres": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32,
                                                     vp, vp, vp, vp, vp, vp]),
     "ddn_resnet34_8s_grad_buckets": (i32, [i32, ctypes.POINTER(i64), i32]),
+    "ddn_net_param_table": (i32, [i32, i32, ctypes.POINTER(TensorEntry), i32]),
+    "ddn_net_buffer_table": (i32, [i32, ctypes.POINTER(TensorEntry), i32]),
+    "ddn_net_param_count": (i64, [i32, i32]),
+    "ddn_net_buffer_count": (i64, [i32]),
+    "ddn_net_workspace_bytes": (sz, [i32] * 7),
+    "ddn_net_weight_cache_bytes": (sz, [i32, i32]),
+    "ddn_net_forward": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, f32, i32, vp, vp]),
+    "ddn_net_backward": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, i32, GRAD_BUCKET_FN, vp, vp]),
+    "ddn_net_grad_buckets": (i32, [i32, i32, ctypes.POINTER(i64), i32]),
     "ddn_contrastive_terms_forward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp, vp]),
     "ddn_contrastive_terms_backward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32,
                                              vp, vp, vp, vp, vp]),
@@ -146,25 +156,30 @@ def require_cuda_f32(t, name, contiguous=True):
         raise RuntimeError("%s must be contiguous" % name)
 
 
-def param_table(D):
-    n = lib.ddn_resnet34_8s_param_table(D, None, 0)
+def param_table(D, arch=ARCH_RESNET34_8S):
+    n = lib.ddn_net_param_table(arch, D, None, 0)
+    check(min(n, 0))
     arr = (TensorEntry * n)()
-    lib.ddn_resnet34_8s_param_table(D, arr, n)
+    lib.ddn_net_param_table(arch, D, arr, n)
     return [(e.name.decode(), tuple(e.shape[:e.ndim]), int(e.offset), int(e.numel)) for e in arr]
 
 
-def buffer_table():
-    n = lib.ddn_resnet34_8s_buffer_table(None, 0)
+def buffer_table(arch=ARCH_RESNET34_8S):
+    n = lib.ddn_net_buffer_table(arch, None, 0)
+    check(min(n, 0))
     arr = (TensorEntry * n)()
-    lib.ddn_resnet34_8s_buffer_table(arr, n)
+    lib.ddn_net_buffer_table(arch, arr, n)
     return [(e.name.decode(), tuple(e.shape[:e.ndim]), int(e.offset), int(e.numel)) for e in arr]
 
 
-def grad_buckets(D):
-    """[(offset, numel)] of the 4 gradient buckets in the order the backward completes them (last layers first)."""
-    arr = (i64 * 5)()
-    n = lib.ddn_resnet34_8s_grad_buckets(D, arr, 5)
-    ends = [int(arr[4])] + [int(arr[i]) for i in range(n - 1)]
+def grad_buckets(D, arch=ARCH_RESNET34_8S):
+    """[(offset, numel)] of the gradient buckets in the order the backward completes them (last layers first); the count is
+    the one the library reports."""
+    n = lib.ddn_net_grad_buckets(arch, D, None, 0)
+    check(min(n, 0))
+    arr = (i64 * (n + 1))()
+    lib.ddn_net_grad_buckets(arch, D, arr, n + 1)
+    ends = [int(arr[n])] + [int(arr[i]) for i in range(n - 1)]
     return [(int(arr[i]), ends[i] - int(arr[i])) for i in range(n)]
 
 

@@ -49,7 +49,11 @@ BnAccum bn_accum_at(void* base, int C) {
   return a;
 }
 
-static inline int bn_rows_per_iter(int C) { return BN_THREADS / (C / 4); }
+// A column-sum block covers at most BN_COLSUM_MAX_C channels (one float4 column per thread); wider tensors are cut into slices
+// of that width along gridDim.z.
+constexpr int BN_COLSUM_MAX_C = 4 * BN_THREADS;
+static inline int bn_slice_c(int C) { return C > BN_COLSUM_MAX_C ? BN_COLSUM_MAX_C : C; }
+static inline int bn_rows_per_iter(int C) { return BN_THREADS / (bn_slice_c(C) / 4); }
 // blocks per group: exactly one resident wave over all groups (`resident` = SMs x CTAs per SM of the kernel, from the occupancy
 // API: a larger grid would run a partial second wave at low occupancy), at least 4 row iterations per block
 static int64_t bn_colsum_rows_per_block(int64_t Mg, int C, int G, int resident) {
@@ -66,6 +70,7 @@ struct BnColsumArgs {
   const float* x; const float* dy; const float* y; const __nv_bfloat16* y_hi;
   const float* mean; const float* invstd; const float* gamma; const float* beta;   // [G][C] statistics (MODE 1)
   int64_t Mg; int C; int64_t rows_per_block; int relu;
+  int Cs;               // channels of one slice (blockIdx.z): C, or BN_COLSUM_MAX_C when C is wider
 };
 
 // column sums of v0, v1 over this block's rows of group blockIdx.y, added into the fp64 accumulator; the last CTA finalizes
@@ -74,8 +79,9 @@ template <int MODE>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_colsum_kernel(BnColsumArgs a, BnFwdFinal ff, BnBwdFinal fb) {
   pdl_prologue();
-  const int C = a.C, q = C >> 2;
-  const int cq = threadIdx.x % q, rr = threadIdx.x / q, rpi = BN_THREADS / q;
+  const int C = a.C, q = a.Cs >> 2;
+  const int rr = threadIdx.x / q, rpi = BN_THREADS / q;
+  const int cq = threadIdx.x % q + (int)blockIdx.z * q;     // float4 column within the full row
   const int g = blockIdx.y;
   const int64_t r0 = (int64_t)g * a.Mg + (int64_t)blockIdx.x * a.rows_per_block;
   const int64_t r1 = min((int64_t)(g + 1) * a.Mg, r0 + a.rows_per_block);
@@ -147,7 +153,7 @@ bn_colsum_kernel(BnColsumArgs a, BnFwdFinal ff, BnBwdFinal fb) {
   double* acc = MODE == 0 ? ff.a.acc : fb.a.acc;
   if (rr == 0) {
     for (int k = 1; k < rpi; ++k) {
-      float4 u = sh0[k * q + cq], w = sh1[k * q + cq];
+      float4 u = sh0[k * q + threadIdx.x], w = sh1[k * q + threadIdx.x];
       s0.x += u.x; s0.y += u.y; s0.z += u.z; s0.w += u.w;
       s1.x += w.x; s1.y += w.y; s1.z += w.z; s1.w += w.w;
     }
@@ -157,7 +163,7 @@ bn_colsum_kernel(BnColsumArgs a, BnFwdFinal ff, BnBwdFinal fb) {
     red_add_f64(p1, (double)s1.x); red_add_f64(p1 + 1, (double)s1.y); red_add_f64(p1 + 2, (double)s1.z); red_add_f64(p1 + 3, (double)s1.w);
   }
   unsigned int* ticket = MODE == 0 ? ff.a.ticket : fb.a.ticket;
-  const bool last = bn_last_cta(ticket, gridDim.x * gridDim.y, threadIdx.x == 0, &s_last, [] { __syncthreads(); });
+  const bool last = bn_last_cta(ticket, gridDim.x * gridDim.y * gridDim.z, threadIdx.x == 0, &s_last, [] { __syncthreads(); });
   if (last) {
     for (int c = threadIdx.x; c < C; c += BN_THREADS) {
       if (MODE == 0) bn_fwd_finalize_channel(ff, c);
@@ -398,8 +404,8 @@ stem_pool_relu_bwd_kernel(const float* __restrict__ dyp, const uint8_t* __restri
 
 // ------------------------------------------------------------------------------------------------ launchers
 static int check_c(int C, int G, int64_t M) {
-  DDN_CHECK_ARG(C >= 4 && C % 4 == 0 && (C / 4) <= BN_THREADS && BN_THREADS % (C / 4) == 0,
-                "BatchNorm kernels need C in {4..1024} with 256 %% (C/4) == 0 (got %d)", C);
+  DDN_CHECK_ARG(C >= 4 && C % 4 == 0 && (C <= BN_COLSUM_MAX_C ? BN_THREADS % (C / 4) == 0 : (C % BN_COLSUM_MAX_C == 0 && C <= 4096)),
+                "BatchNorm kernels need C in {4..1024} with 256 %% (C/4) == 0, or a multiple of 1024 up to 4096 (got %d)", C);
   DDN_CHECK_ARG(G >= 1 && G <= BN_MAX_GROUPS && M % G == 0, "BatchNorm groups: need 1 <= G <= %d dividing the row count", BN_MAX_GROUPS);
   return 0;
 }
@@ -422,10 +428,11 @@ int launch_bn_stats(const float* x, int64_t M, int C, int G, BnAccum acc, float*
   DDN_TRY(check_c(C, G, M));
   const int64_t Mg = M / G;
   const int resident = resident_blocks(bn_colsum_kernel<0>, 0);
-  BnColsumArgs a = {x, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, Mg, C, bn_colsum_rows_per_block(Mg, C, G, resident), 0};
+  const int Cs = bn_slice_c(C), slices = C / Cs;
+  BnColsumArgs a = {x, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, Mg, C, bn_colsum_rows_per_block(Mg, C, G * slices, resident), 0, Cs};
   BnFwdFinal ff = {acc, mean, invstd, running_mean, running_var, Mg, G, C, momentum, eps};
   BnBwdFinal fb = {};
-  dim3 grid((unsigned)bn_colsum_blocks(Mg, C, G, resident), (unsigned)G);
+  dim3 grid((unsigned)bn_colsum_blocks(Mg, C, G * slices, resident), (unsigned)G, (unsigned)slices);
   DDN_LAUNCH(bn_colsum_kernel<0>, grid, BN_THREADS, 0, st, a, ff, fb);
   return 0;
 }
@@ -436,11 +443,13 @@ int launch_bn_eval_stats(const float* rm, const float* rv, int C, int G, float e
 }
 
 int launch_bn_eval_stats_all(const float* buffers, float* stats_base, const BnEvalSeg* segs, int n_segs, int G, float eps, cudaStream_t st) {
-  DDN_CHECK_ARG(n_segs >= 1 && n_segs <= BN_EVAL_MAX_SEGS, "too many BatchNorm segments");
-  BnEvalSegs s; s.n = n_segs;
-  for (int i = 0; i < n_segs; ++i) s.s[i] = segs[i];
-  dim3 grid(2, (unsigned)n_segs);
-  DDN_LAUNCH(bn_eval_stats_all_kernel, grid, 256, 0, st, buffers, stats_base, s, G, eps);
+  DDN_CHECK_ARG(n_segs >= 1, "no BatchNorm segments");
+  for (int i0 = 0; i0 < n_segs; i0 += BN_EVAL_MAX_SEGS) {     // one launch per table slice
+    BnEvalSegs s; s.n = std::min(BN_EVAL_MAX_SEGS, n_segs - i0);
+    for (int i = 0; i < s.n; ++i) s.s[i] = segs[i0 + i];
+    dim3 grid(2, (unsigned)s.n);
+    DDN_LAUNCH(bn_eval_stats_all_kernel, grid, 256, 0, st, buffers, stats_base, s, G, eps);
+  }
   return 0;
 }
 
@@ -450,9 +459,17 @@ int launch_bn_fold(const float* rm, const float* rv, const float* gamma, const f
   return 0;
 }
 
+// the per-channel tables of the apply kernels exceed the default 48 KB of dynamic shared memory above C = 512 (G = 2)
+template <typename K>
+static int allow_smem(K kernel, size_t smem) {
+  if (smem > 48 * 1024) DDN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return 0;
+}
+
 int launch_bn_apply(const BnApplyArgs& a, cudaStream_t st) {
   DDN_TRY(check_c(a.C, a.G, a.M));
   const size_t smem = (size_t)a.G * ((a.r && a.rmean) ? 6 : 3) * a.C * sizeof(float);
+  DDN_TRY(allow_smem(bn_apply_kernel, smem));
   DDN_LAUNCH(bn_apply_kernel, ew_blocks(bn_apply_kernel, smem, a.M * (a.C / 4)), BN_THREADS, smem, st, a);
   return 0;
 }
@@ -461,13 +478,16 @@ int launch_bn_backward(const BnBwdArgs& a, cudaStream_t st) {
   DDN_TRY(check_c(a.C, a.G, a.M));
   const int64_t Mg = a.M / a.G;
   const int resident = resident_blocks(bn_colsum_kernel<1>, 0);
-  BnColsumArgs ca = {a.x, a.dy, a.y, a.y_hi, a.mean, a.invstd, a.gamma, a.beta, Mg, a.C, bn_colsum_rows_per_block(Mg, a.C, a.G, resident), a.relu};
+  const int Cs = bn_slice_c(a.C), slices = a.C / Cs;
+  BnColsumArgs ca = {a.x, a.dy, a.y, a.y_hi, a.mean, a.invstd, a.gamma, a.beta, Mg, a.C, bn_colsum_rows_per_block(Mg, a.C, a.G * slices, resident),
+                     a.relu, Cs};
   DDN_CHECK_ARG(!(a.relu && !a.y && !a.y_hi) || a.beta, "recomputing the ReLU mask needs beta");
   BnFwdFinal ff = {};
   BnBwdFinal fb = {a.acc, a.sums, a.dgamma, a.dbeta, a.G, a.C};
-  dim3 grid((unsigned)bn_colsum_blocks(Mg, a.C, a.G, resident), (unsigned)a.G);
+  dim3 grid((unsigned)bn_colsum_blocks(Mg, a.C, a.G * slices, resident), (unsigned)a.G, (unsigned)slices);
   if (!a.sums_ready) DDN_LAUNCH(bn_colsum_kernel<1>, grid, BN_THREADS, 0, st, ca, ff, fb);
   const size_t smem = (size_t)a.G * 7 * a.C * sizeof(float);
+  DDN_TRY(allow_smem(bn_bwd_apply_kernel, smem));
   DDN_LAUNCH(bn_bwd_apply_kernel, ew_blocks(bn_bwd_apply_kernel, smem, a.M * (a.C / 4)), BN_THREADS, smem, st, a);
   return 0;
 }

@@ -1510,6 +1510,7 @@ bool tc_conv_supported(int Cin, int Cout, int k, int stride, int pad, int dil, i
 }
 
 static const size_t kMaxWeightElems = (size_t)9 * 512 * 512;
+size_t tc_max_weight_elems() { return kMaxWeightElems; }
 size_t tc_weight_ws_bytes() { return 2 * align_up(kMaxWeightElems * 2, 1024) + 2048; }
 
 int tc_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, int precision, cudaStream_t st) {
@@ -1722,12 +1723,14 @@ int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1,
 // stored at `fp_old` (or `force`): three launches, no host synchronisation.  fp_new / fp_old: 2 x uint64 each, fp_new zero.
 int tc_pack_all(const float* params, int64_t n_params, char* cache, const TcPackEntry* entries, int n, unsigned long long* fp_new,
                 unsigned long long* fp_old, int force, int precision, cudaStream_t st) {
-  DDN_CHECK_ARG(n >= 1 && n <= TC_PACK_MAX, "pack table too large");
-  TcPackTable t; t.n = n;
-  for (int i = 0; i < n; ++i) t.e[i] = entries[i];
+  DDN_CHECK_ARG(n >= 1, "empty pack table");
   DDN_LAUNCH(param_fingerprint_kernel, num_sms() * 2, 256, 0, st, reinterpret_cast<const uint32_t*>(params), n_params, fp_new);
-  dim3 grid(32, (unsigned)n);
-  DDN_LAUNCH(pack_all_kernel, grid, 256, 0, st, params, cache, t, fp_new, fp_old, force, precision == DDN_PRECISION_BF16X3 ? 1 : 0);
+  for (int i0 = 0; i0 < n; i0 += TC_PACK_MAX) {     // a table longer than one launch's parameter block: one launch per slice
+    TcPackTable t; t.n = std::min(TC_PACK_MAX, n - i0);
+    for (int i = 0; i < t.n; ++i) t.e[i] = entries[i0 + i];
+    dim3 grid(32, (unsigned)t.n);
+    DDN_LAUNCH(pack_all_kernel, grid, 256, 0, st, params, cache, t, fp_new, fp_old, force, precision == DDN_PRECISION_BF16X3 ? 1 : 0);
+  }
   DDN_LAUNCH(commit_fingerprint_kernel, 1, 32, 0, st, fp_new, fp_old);
   return 0;
 }

@@ -27,6 +27,7 @@ struct TcBwdStats {
 // forward / weight gradient: 3x3 (pad == dil) or 1x1 (pad 0), Cin and Cout multiples of 64, stride 1 (any dil) or 2 (dil 1)
 bool tc_conv_supported(int Cin, int Cout, int k, int stride, int pad, int dil, int H, int W);
 size_t tc_weight_ws_bytes();                       // staging for one conv's packed bf16 weights
+size_t tc_max_weight_elems();                      // the largest weight tensor (Cout*Cin*k*k) that staging holds
 size_t tc_workspace_bytes(size_t max_act_elems);   // staging for the fp32-tensor wrappers below
 int tc_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, int precision, cudaStream_t st);
 

@@ -1,10 +1,11 @@
-// Network-level orchestration of Resnet34_8s forward/backward behind the C ABI, plus the single-operator
+// Network-level orchestration of the dilated backbones' forward/backward behind the C ABI, plus the single-operator
 // entry points.  The structure restated here is the reference's
-//   PSD/vision/torchvision/models/resnet.py:112-265  (ResNet.__init__/_make_layer/forward, BasicBlock)
-//   PSD/pytorch_segmentation_detection/models/resnet_dilated.py:283-322 (Resnet34_8s)
-// configured as resnet34(fully_conv=True, output_stride=8, remove_avg_pool_layer=True).
+//   PSD/vision/torchvision/models/resnet.py:112-265  (ResNet.__init__/_make_layer/forward, BasicBlock :53-69, Bottleneck :72-109)
+//   PSD/pytorch_segmentation_detection/models/resnet_dilated.py:283-322 (Resnet34_8s), :399-435 (Resnet50_8s)
+// configured as resnet34 / resnet50(fully_conv=True, output_stride=8, remove_avg_pool_layer=True).
 #include <algorithm>
 #include <cstring>
+#include <deque>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -86,12 +87,17 @@ ProfScope::~ProfScope() {
 // ------------------------------------------------------------------------------------------------ network description
 struct ConvSpec { int cin, cout, k, stride, pad, dil; int64_t w_off; };
 struct BnSpec { int C; int64_t g_off, b_off, rm_off, rv_off; };
-struct BlockSpec { ConvSpec c1, c2, ds; BnSpec b1, b2, bd; bool has_ds; };
+// main branch: c[0..n) each followed by b[0..n) (ReLU after all but the last, which takes the residual first);
+// BasicBlock: n = 2 (3x3, 3x3), Bottleneck: n = 3 (1x1, 3x3 carrying the stride and dilation, 1x1 expanding to 4 x planes)
+struct BlockSpec { int n; ConvSpec c[3], ds; BnSpec b[3], bd; bool has_ds; };
 
 struct NetSpec {
-  int D = 0;
+  int arch = 0, D = 0;
   ConvSpec stem; BnSpec stem_bn;
   std::vector<BlockSpec> blocks;
+  int layer_first[4] = {0, 0, 0, 0};    // index of each residual layer's first block
+  int max_c = 0;                        // widest BatchNorm (sizes the statistics accumulator and the column-sum slots)
+  int fc_cin = 0;                       // channels of the trunk output (the fc input)
   int64_t fc_w = 0, fc_b = 0, n_params = 0, n_buffers = 0;
   std::vector<ddn_tensor_entry> ptab, btab;
 };
@@ -110,8 +116,10 @@ static void add_entry(std::vector<ddn_tensor_entry>& tab, int64_t& cursor, const
   tab.push_back(e);
 }
 
-static NetSpec build_spec(int D) {
-  NetSpec s; s.D = D;
+static NetSpec build_spec(int arch, int D) {
+  NetSpec s; s.arch = arch; s.D = D;
+  const bool bottleneck = arch == DDN_ARCH_RESNET50_8S;
+  const int expansion = bottleneck ? 4 : 1;
   int64_t pc = 0, bc = 0;
   auto conv = [&](const std::string& name, int cin, int cout, int k, int stride, int pad, int dil) {
     ConvSpec c{cin, cout, k, stride, pad, dil, 0};
@@ -133,41 +141,58 @@ static NetSpec build_spec(int D) {
   int inplanes = 64, current_stride = 4, current_dilation = 1;
   for (int L = 0; L < 4; ++L) {
     int stride = strides[L];
-    bool ds = stride != 1 || inplanes != planes[L];
+    const int out_c = planes[L] * expansion;
+    bool ds = stride != 1 || inplanes != out_c;
     if (ds) {
       if (current_stride == 8) { current_dilation *= stride; stride = 1; }
       else current_stride *= stride;
     }
+    s.layer_first[L] = (int)s.blocks.size();
     for (int i = 0; i < layers[L]; ++i) {
       std::string p = "layer" + std::to_string(L + 1) + "." + std::to_string(i);
       BlockSpec b; memset(&b, 0, sizeof(b));
       int st = i == 0 ? stride : 1;
       int dil = current_dilation;
-      b.c1 = conv(p + ".conv1", inplanes, planes[L], 3, st, dil, dil);
-      b.b1 = bn(p + ".bn1", planes[L]);
-      b.c2 = conv(p + ".conv2", planes[L], planes[L], 3, 1, dil, dil);
-      b.b2 = bn(p + ".bn2", planes[L]);
+      if (bottleneck) {       // resnet.py:72-109: the stride sits on conv2, the 3x3
+        b.n = 3;
+        b.c[0] = conv(p + ".conv1", inplanes, planes[L], 1, 1, 0, 1);
+        b.b[0] = bn(p + ".bn1", planes[L]);
+        b.c[1] = conv(p + ".conv2", planes[L], planes[L], 3, st, dil, dil);
+        b.b[1] = bn(p + ".bn2", planes[L]);
+        b.c[2] = conv(p + ".conv3", planes[L], out_c, 1, 1, 0, 1);
+        b.b[2] = bn(p + ".bn3", out_c);
+      } else {
+        b.n = 2;
+        b.c[0] = conv(p + ".conv1", inplanes, planes[L], 3, st, dil, dil);
+        b.b[0] = bn(p + ".bn1", planes[L]);
+        b.c[1] = conv(p + ".conv2", planes[L], planes[L], 3, 1, dil, dil);
+        b.b[1] = bn(p + ".bn2", planes[L]);
+      }
       b.has_ds = (i == 0) && ds;
       if (b.has_ds) {
-        b.ds = conv(p + ".downsample.0", inplanes, planes[L], 1, st, 0, 1);
-        b.bd = bn(p + ".downsample.1", planes[L]);
+        b.ds = conv(p + ".downsample.0", inplanes, out_c, 1, st, 0, 1);
+        b.bd = bn(p + ".downsample.1", out_c);
       }
       s.blocks.push_back(b);
-      inplanes = planes[L];
+      inplanes = out_c;
+      s.max_c = std::max(s.max_c, out_c);
     }
   }
-  add_entry(s.ptab, pc, "fc.weight", {D, 512, 1, 1}, &s.fc_w);
+  s.fc_cin = inplanes;
+  add_entry(s.ptab, pc, "fc.weight", {D, inplanes, 1, 1}, &s.fc_w);
   add_entry(s.ptab, pc, "fc.bias", {D}, &s.fc_b);
   s.n_params = pc; s.n_buffers = bc;
   return s;
 }
 
-static const NetSpec& get_spec(int D) {
+static bool arch_ok(int arch) { return arch == DDN_ARCH_RESNET34_8S || arch == DDN_ARCH_RESNET50_8S; }
+
+static const NetSpec& get_spec(int arch, int D) {
   static std::mutex mu;
-  static std::vector<NetSpec> cache;
+  static std::deque<NetSpec> cache;       // a deque: references handed out stay valid when it grows
   std::lock_guard<std::mutex> lk(mu);
-  for (auto& s : cache) if (s.D == D) return s;
-  cache.push_back(build_spec(D));
+  for (auto& s : cache) if (s.arch == arch && s.D == D) return s;
+  cache.push_back(build_spec(arch, D));
   return cache.back();
 }
 
@@ -177,9 +202,10 @@ static const NetSpec& get_spec(int D) {
 // backpropagates through an eval()-mode network this way).
 struct ConvBufs { size_t raw, stats; int Hin, Win, Hout, Wout; };   // stats: [G][C] mean, then [G][C] 1/sqrt(var+eps)
 struct PlaneBufs { size_t hi, lo; };   // bf16 operand planes of an activation (tensor-core modes only)
-struct BlockBufs { ConvBufs c1, c2, ds; size_t act1, out; PlaneBufs act1_p, out_p; };
+// act[j] / act_p[j]: relu(bn(c[j])) for j < n-1 (the input of c[j+1]); out / out_p: the block output
+struct BlockBufs { ConvBufs c[3], ds; size_t act[2], out; PlaneBufs act_p[2], out_p; };
 struct Plan {
-  int B, H, W, D, mode, precision;
+  int arch, B, H, W, D, mode, precision;
   int H1, W1, Hp, Wp;
   size_t x4, stem_raw, stem_stats, pool_out, argmax;
   PlaneBufs pool_p, grad_p, patch_p;  // pooled stem output; current d(raw conv output); 7x7/2 stem patches [B,H1,W1,192]
@@ -188,7 +214,7 @@ struct Plan {
   std::vector<BlockBufs> blk;
   size_t low, dlow;
   size_t wpack, wpack2, dwp, scratch[4];
-  size_t fc_part;                     // FC_PART_SLOTS x (D*512 + D) floats: per-block partial sums of the fc gradient
+  size_t fc_part;                     // fc_part_floats(C, D) floats: per-block partial sums of the fc gradient
   size_t acc, sums;                   // BatchNorm accumulator (bn_stats.cuh) and the backward's per-group sums
   size_t dwp_all;                     // [n_params + 64*192] doubles: every conv's [taps][Cout][Cin] gradient accumulator (tensor-core modes)
   size_t scratch_elems;
@@ -197,13 +223,14 @@ struct Plan {
 
 static float* stat_mean(char* ws, const ConvBufs& cb) { return reinterpret_cast<float*>(ws + cb.stats); }
 
-static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precision) {
+static int make_plan(Plan* p, int arch, int B, int H, int W, int D, int mode, int precision) {
+  DDN_CHECK_ARG(arch_ok(arch), "unknown architecture id %d", arch);
   DDN_CHECK_ARG(B >= 1 && H >= 32 && W >= 32 && H % 8 == 0 && W % 8 == 0, "need B>=1 and H, W multiples of 8 (>=32); got B=%d H=%d W=%d", B, H, W);
   DDN_CHECK_ARG(D >= 1 && D <= 32, "descriptor dimension must be in [1,32] (got %d)", D);
   DDN_CHECK_ARG(precision >= DDN_PRECISION_FP32_SIMT && precision <= DDN_PRECISION_BF16, "unknown precision %d", precision);
   DDN_CHECK_ARG(mode >= DDN_MODE_INFER && mode <= DDN_MODE_EVAL_SAVE, "unknown mode %d", mode);
-  const NetSpec& s = get_spec(D);
-  p->B = B; p->H = H; p->W = W; p->D = D; p->mode = mode; p->precision = precision;
+  const NetSpec& s = get_spec(arch, D);
+  p->arch = arch; p->B = B; p->H = H; p->W = W; p->D = D; p->mode = mode; p->precision = precision;
   const int G = BN_MAX_GROUPS;
   size_t cur = 0;
   auto alloc = [&](size_t bytes) { size_t o = cur; cur += align_up(bytes, 256); return o; };
@@ -223,36 +250,55 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
   int h = p->Hp, w = p->Wp;
   size_t max_w = 0;
   int64_t max_act = (int64_t)B * p->H1 * p->W1 * 64;
+  int64_t max_up = 0;
   p->blk.clear();
   for (const BlockSpec& b : s.blocks) {
     BlockBufs bb;
     memset(&bb, 0, sizeof(bb));
+    size_t blk_max_w = 0;
     auto conv_bufs = [&](const ConvSpec& c, int hin, int win) {
       ConvBufs cb; cb.Hin = hin; cb.Win = win;
       cb.Hout = (hin + 2 * c.pad - c.dil * (c.k - 1) - 1) / c.stride + 1;
       cb.Wout = (win + 2 * c.pad - c.dil * (c.k - 1) - 1) / c.stride + 1;
       cb.raw = f32((int64_t)B * cb.Hout * cb.Wout * c.cout);
       cb.stats = f32(2 * G * c.cout);
-      max_w = std::max(max_w, (size_t)c.k * c.k * c.cin * c.cout);
+      blk_max_w = std::max(blk_max_w, (size_t)c.k * c.k * c.cin * c.cout);
       max_act = std::max(max_act, (int64_t)B * cb.Hout * cb.Wout * c.cout);
+      // the data gradient of a strided conv zero-inserts dY [B, Hin, Win, Cout] into the gradient planes (only those)
+      if (c.stride == 2) max_up = std::max(max_up, (int64_t)B * hin * win * c.cout);
       return cb;
     };
-    bb.c1 = conv_bufs(b.c1, h, w);
-    // tensor-core modes keep activations only as bf16 hi/lo planes; the fp32 SIMT instrument keeps fp32 tensors
-    if (!p->tc) bb.act1 = f32((int64_t)B * bb.c1.Hout * bb.c1.Wout * b.c1.cout);
-    bb.act1_p = planes((int64_t)B * bb.c1.Hout * bb.c1.Wout * b.c1.cout);
-    bb.c2 = conv_bufs(b.c2, bb.c1.Hout, bb.c1.Wout);
-    if (b.has_ds) bb.ds = conv_bufs(b.ds, h, w);
-    if (!p->tc) bb.out = f32((int64_t)B * bb.c2.Hout * bb.c2.Wout * b.c2.cout);
-    bb.out_p = planes((int64_t)B * bb.c2.Hout * bb.c2.Wout * b.c2.cout);
+    const int last = b.n - 1;
+    int hc = h, wc = w;
+    for (int j = 0; j < b.n; ++j) {
+      bb.c[j] = conv_bufs(b.c[j], hc, wc);
+      hc = bb.c[j].Hout; wc = bb.c[j].Wout;
+      const int64_t n_el = (int64_t)B * hc * wc * b.c[j].cout;
+      // tensor-core modes keep activations only as bf16 hi/lo planes; the fp32 SIMT instrument keeps fp32 tensors
+      if (j < last) {
+        if (!p->tc) bb.act[j] = f32(n_el);
+        bb.act_p[j] = planes(n_el);
+      }
+      if (j == last && b.has_ds) bb.ds = conv_bufs(b.ds, h, w);
+    }
+    if (!p->tc) bb.out = f32((int64_t)B * hc * wc * b.c[last].cout);
+    bb.out_p = planes((int64_t)B * hc * wc * b.c[last].cout);
     // a tensor-core plan keeps no fp32 activations, so every block conv must have a tensor-core kernel (true for every H, W
     // accepted above; a change of the spec or of that rule becomes an error here instead of a null read in a SIMT conv)
     auto on_tc = [&](const ConvSpec& c, const ConvBufs& cb) { return tc_conv_supported(c.cin, c.cout, c.k, c.stride, c.pad, c.dil, cb.Hin, cb.Win); };
-    if (p->tc && !(on_tc(b.c1, bb.c1) && on_tc(b.c2, bb.c2) && (!b.has_ds || on_tc(b.ds, bb.ds)))) {
+    bool all_tc = !b.has_ds || on_tc(b.ds, bb.ds);
+    for (int j = 0; j < b.n; ++j) all_tc = all_tc && on_tc(b.c[j], bb.c[j]);
+    if (p->tc && !all_tc) {
       set_error("a block convolution at %dx%d has no tensor-core kernel (precision %d)", h, w, precision);
       return DDN_EUNSUPPORTED;
     }
-    h = bb.c2.Hout; w = bb.c2.Wout;
+    // the packed weights of a conv without a cached pack are staged in a fixed-size area (conv_tc.cu)
+    if (p->tc && blk_max_w > tc_max_weight_elems()) {
+      set_error("a block convolution has %zu weights, more than the %zu the tensor-core weight staging holds", blk_max_w, tc_max_weight_elems());
+      return DDN_EUNSUPPORTED;
+    }
+    max_w = std::max(max_w, blk_max_w);
+    h = hc; w = wc;
     p->blk.push_back(bb);
   }
   DDN_CHECK_ARG(h * 8 == H && w * 8 == W, "internal: trunk output %dx%d is not H/8 x W/8", h, w);
@@ -260,14 +306,14 @@ static int make_plan(Plan* p, int B, int H, int W, int D, int mode, int precisio
   p->dlow = f32((int64_t)B * D * h * w);
   max_w = std::max(max_w, (size_t)7 * 7 * 4 * 64);
   p->wpack = f32((int64_t)max_w); p->wpack2 = f32((int64_t)max_w); p->dwp = f32((int64_t)max_w);
-  p->acc = alloc(bn_accum_bytes(512));
-  p->sums = f32(3 * 2 * G * 512);     // [0]: standalone column-sum pass, [1], [2]: sums produced by a data-gradient epilogue
+  p->acc = alloc(bn_accum_bytes(s.max_c));
+  p->sums = f32(3 * 2 * G * s.max_c);     // [0]: standalone column-sum pass, [1], [2]: sums produced by a data-gradient epilogue
   p->scratch_elems = (size_t)max_act;
   for (int i = 0; i < 4; ++i) p->scratch[i] = f32((int64_t)max_act);
-  p->grad_p = planes(max_act);
+  p->grad_p = planes(std::max(max_act, max_up));
   p->wws = alloc(p->tc ? tc_weight_ws_bytes() : 0);
   p->dwp_all = (p->tc && mode != DDN_MODE_INFER) ? alloc(sizeof(double) * (size_t)(s.n_params + 64 * 192)) : 0;
-  p->fc_part = mode != DDN_MODE_INFER ? f32((int64_t)FC_PART_SLOTS * (D * 512 + D)) : 0;
+  p->fc_part = mode != DDN_MODE_INFER ? f32((int64_t)fc_part_floats(s.fc_cin, D)) : 0;
   p->total = cur;
   return 0;
 }
@@ -281,7 +327,8 @@ struct Ctx {
   TcPlanes planes(const PlaneBufs& b) const { return TcPlanes{h(b.hi), h(b.lo)}; }
   float* mean(size_t stats) const { return f(stats); }
   float* invstd(size_t stats, int C) const { return f(stats) + (size_t)G * C; }
-  BnAccum accum() const { return bn_accum_at(ws + p->acc, 512); }
+  BnAccum accum() const { return bn_accum_at(ws + p->acc, s->max_c); }
+  float* sums(int slot) const { return f(p->sums) + (size_t)slot * 2 * G * s->max_c; }
   bool training() const { return mode == DDN_MODE_TRAIN; }
 };
 
@@ -321,7 +368,7 @@ static int ensure_packs(const Ctx& c) {
   };
   add(s.stem, 0, 1);
   for (const BlockSpec& b : s.blocks) {
-    add(b.c1, 0, 0); add(b.c1, 1, 0); add(b.c2, 0, 0); add(b.c2, 1, 0);
+    for (int j = 0; j < b.n; ++j) { add(b.c[j], 0, 0); add(b.c[j], 1, 0); }
     if (b.has_ds) { add(b.ds, 0, 0); add(b.ds, 1, 0); }
   }
   unsigned long long* fp_new = reinterpret_cast<unsigned long long*>(wc->base + wc->bytes - 256);
@@ -407,7 +454,7 @@ static int fill_eval_stats(const Ctx& c) {
   };
   add(s.stem_bn, p.stem_stats);
   for (size_t i = 0; i < s.blocks.size(); ++i) {
-    add(s.blocks[i].b1, p.blk[i].c1.stats); add(s.blocks[i].b2, p.blk[i].c2.stats);
+    for (int j = 0; j < s.blocks[i].n; ++j) add(s.blocks[i].b[j], p.blk[i].c[j].stats);
     if (s.blocks[i].has_ds) add(s.blocks[i].bd, p.blk[i].ds.stats);
   }
   return launch_bn_eval_stats_all(c.buffers, reinterpret_cast<float*>(c.ws), segs.data(), (int)segs.size(), c.G, c.eps, c.st);
@@ -418,7 +465,7 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   const int B = p.B, G = c.G;
   const bool want_lo = p.precision == DDN_PRECISION_BF16X3;
   const bool fold = c.mode == DDN_MODE_INFER && p.tc;
-  DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(512), c.st));     // the workspace arrives uninitialised
+  DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(s.max_c), c.st));     // the workspace arrives uninitialised
   if (p.tc) DDN_TRY(ensure_packs(c));
   if (!c.training() && !fold) DDN_TRY(fill_eval_stats(c));
   // stem: conv1 7x7/2 -> bn1 -> relu -> maxpool 3x3/2          (resnet.py:232-235)
@@ -441,38 +488,47 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
                                    B, p.H1, p.W1, 64, G, c.st));
   const float* cur = p.tc ? nullptr : c.f(p.pool_out);      // fp32 activations exist only in the SIMT instrument
   PlaneBufs cur_p = p.pool_p;
-  for (size_t i = 0; i < s.blocks.size(); ++i) {        // BasicBlock.forward, resnet.py:53-69
+  for (size_t i = 0; i < s.blocks.size(); ++i) {        // BasicBlock.forward, resnet.py:53-69 / Bottleneck.forward, :87-109
     const BlockSpec& b = s.blocks[i]; const BlockBufs& bb = p.blk[i];
-    int64_t M1 = (int64_t)B * bb.c1.Hout * bb.c1.Wout;
+    const int last = b.n - 1;
     if (fold) {
-      DDN_TRY(conv_bn_folded(c, b.c1, b.b1, cur_p, bb.c1, B, nullptr, &bb.act1_p, nullptr, 1));       // act1: planes only
+      PlaneBufs in_p = cur_p;
+      for (int j = 0; j < last; ++j) {     // act[j]: planes only
+        DDN_TRY(conv_bn_folded(c, b.c[j], b.b[j], in_p, bb.c[j], B, nullptr, &bb.act_p[j], nullptr, 1));
+        in_p = bb.act_p[j];
+      }
       // the epilogue's residual addend is fp32: the pooled stem output for the first block, else the previous block's fp32
-      // output, which the folded path keeps in that block's (otherwise unused) c2.raw slot
-      const float* res = i == 0 ? c.f(p.pool_out) : c.f(p.blk[i - 1].c2.raw);
+      // output, which the folded path keeps in that block's (otherwise unused) last raw slot
+      const float* res = i == 0 ? c.f(p.pool_out) : c.f(p.blk[i - 1].c[last].raw);
       if (b.has_ds) {
         DDN_TRY(conv_bn_folded(c, b.ds, b.bd, cur_p, bb.ds, B, c.f(bb.ds.raw), nullptr, nullptr, 0));  // bn_d(conv_d(x)), fp32
         res = c.f(bb.ds.raw);
       }
-      DDN_TRY(conv_bn_folded(c, b.c2, b.b2, bb.act1_p, bb.c2, B, c.f(bb.c2.raw), &bb.out_p, res, 1));   // fp32 block output in c2.raw
-      cur = c.f(bb.c2.raw);
+      DDN_TRY(conv_bn_folded(c, b.c[last], b.b[last], in_p, bb.c[last], B, c.f(bb.c[last].raw), &bb.out_p, res, 1));   // fp32 block output
+      cur = c.f(bb.c[last].raw);
       cur_p = bb.out_p;
       continue;
     }
-    DDN_TRY(conv_bn_forward(c, b.c1, b.b1, cur, cur_p, bb.c1, B, b.c1.cin));
-    BnApplyArgs a1;
-    memset(&a1, 0, sizeof(a1));
-    a1.x = c.f(bb.c1.raw); a1.mean = c.mean(bb.c1.stats); a1.invstd = c.invstd(bb.c1.stats, b.b1.C);
-    a1.gamma = c.params + b.b1.g_off; a1.beta = c.params + b.b1.b_off;
-    a1.y = p.tc ? nullptr : c.f(bb.act1); a1.hi = p.tc ? c.h(bb.act1_p.hi) : nullptr; a1.lo = (p.tc && want_lo) ? c.h(bb.act1_p.lo) : nullptr;
-    a1.M = M1; a1.C = b.b1.C; a1.relu = 1; a1.G = G;
-    DDN_TRY(launch_bn_apply(a1, c.st));
-    DDN_TRY(conv_bn_forward(c, b.c2, b.b2, p.tc ? nullptr : c.f(bb.act1), bb.act1_p, bb.c2, B, b.c2.cin));
+    const float* in = cur; PlaneBufs in_p = cur_p;
+    for (int j = 0; j < last; ++j) {       // act[j] = relu(bn_j(conv_j(in)))
+      DDN_TRY(conv_bn_forward(c, b.c[j], b.b[j], in, in_p, bb.c[j], B, b.c[j].cin));
+      BnApplyArgs a1;
+      memset(&a1, 0, sizeof(a1));
+      a1.x = c.f(bb.c[j].raw); a1.mean = c.mean(bb.c[j].stats); a1.invstd = c.invstd(bb.c[j].stats, b.b[j].C);
+      a1.gamma = c.params + b.b[j].g_off; a1.beta = c.params + b.b[j].b_off;
+      a1.y = p.tc ? nullptr : c.f(bb.act[j]); a1.hi = p.tc ? c.h(bb.act_p[j].hi) : nullptr;
+      a1.lo = (p.tc && want_lo) ? c.h(bb.act_p[j].lo) : nullptr;
+      a1.M = (int64_t)B * bb.c[j].Hout * bb.c[j].Wout; a1.C = b.b[j].C; a1.relu = 1; a1.G = G;
+      DDN_TRY(launch_bn_apply(a1, c.st));
+      in = p.tc ? nullptr : c.f(bb.act[j]); in_p = bb.act_p[j];
+    }
+    DDN_TRY(conv_bn_forward(c, b.c[last], b.b[last], in, in_p, bb.c[last], B, b.c[last].cin));
     BnApplyArgs a2;
     memset(&a2, 0, sizeof(a2));
-    a2.x = c.f(bb.c2.raw); a2.mean = c.mean(bb.c2.stats); a2.invstd = c.invstd(bb.c2.stats, b.b2.C);
-    a2.gamma = c.params + b.b2.g_off; a2.beta = c.params + b.b2.b_off;
+    a2.x = c.f(bb.c[last].raw); a2.mean = c.mean(bb.c[last].stats); a2.invstd = c.invstd(bb.c[last].stats, b.b[last].C);
+    a2.gamma = c.params + b.b[last].g_off; a2.beta = c.params + b.b[last].b_off;
     a2.y = p.tc ? nullptr : c.f(bb.out); a2.hi = p.tc ? c.h(bb.out_p.hi) : nullptr; a2.lo = (p.tc && want_lo) ? c.h(bb.out_p.lo) : nullptr;
-    a2.M = M1; a2.C = b.b2.C; a2.relu = 1; a2.G = G;
+    a2.M = (int64_t)B * bb.c[last].Hout * bb.c[last].Wout; a2.C = b.b[last].C; a2.relu = 1; a2.G = G;
     if (b.has_ds) {
       DDN_TRY(conv_bn_forward(c, b.ds, b.bd, cur, cur_p, bb.ds, B, b.ds.cin));
       a2.r = c.f(bb.ds.raw); a2.rmean = c.mean(bb.ds.stats); a2.rinvstd = c.invstd(bb.ds.stats, b.bd.C);
@@ -491,7 +547,7 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   const bool feat_planes = p.tc;       // the features are read from the operand planes (hi + lo)
   DDN_TRY(launch_fc_forward(feat_planes ? nullptr : cur, feat_planes ? c.h(cur_p.hi) : nullptr,
                             (feat_planes && want_lo) ? c.h(cur_p.lo) : nullptr, c.params + s.fc_w, c.params + s.fc_b, c.f(p.low),
-                            low_nhwc, (int64_t)h8 * w8, B, 512, p.D, c.st));
+                            low_nhwc, (int64_t)h8 * w8, B, s.fc_cin, p.D, c.st));
   DDN_TRY(launch_upsample_fwd(c.f(p.low), y, B * p.D, h8, w8, p.H, p.W, c.st));
   return 0;
 }
@@ -551,7 +607,7 @@ static int bn_backward_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, c
   a.gamma = c.params + bs.g_off; a.beta = c.params + bs.b_off;
   a.y = y_f32; a.y_hi = y_hi; a.g_out = g_out;
   a.dgamma = c.grads + bs.g_off; a.dbeta = c.grads + bs.b_off;
-  a.acc = c.accum(); a.sums = c.f(c.p->sums) + (size_t)fused_slot * 2 * c.G * 512;
+  a.acc = c.accum(); a.sums = c.sums(fused_slot);
   a.sums_ready = fused_slot > 0;
   a.M = M; a.C = bs.C; a.relu = relu; a.training = c.training() ? 1 : 0; a.G = c.G;
   if (c.p->tc) {
@@ -571,7 +627,7 @@ static bool bwd_stats_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, co
   memset(out, 0, sizeof(*out));
   out->raw = c.f(cb.raw); out->y_hi = y_hi; out->mean = c.mean(cb.stats); out->invstd = c.invstd(cb.stats, bs.C);
   out->gamma = c.params + bs.g_off; out->beta = c.params + bs.b_off; out->relu = 1;
-  out->fin.a = c.accum(); out->fin.sums = c.f(c.p->sums) + (size_t)slot * 2 * c.G * 512;
+  out->fin.a = c.accum(); out->fin.sums = c.sums(slot);
   out->fin.dgamma = c.grads + bs.g_off; out->fin.dbeta = c.grads + bs.b_off; out->fin.G = c.G; out->fin.C = bs.C;
   return true;
 }
@@ -584,7 +640,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   const int B = p.B, h8 = p.H / 8, w8 = p.W / 8;
   const bool want_lo = p.precision == DDN_PRECISION_BF16X3;
   float* S[4] = {c.f(p.scratch[0]), c.f(p.scratch[1]), c.f(p.scratch[2]), c.f(p.scratch[3])};
-  DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(512), c.st));
+  DDN_CUDA(cudaMemsetAsync(c.ws + p.acc, 0, bn_accum_bytes(s.max_c), c.st));
   if (p.tc) DDN_CUDA(cudaMemsetAsync(c.d(p.dwp_all), 0, sizeof(double) * (size_t)(s.n_params + 64 * 192), c.st));
   const BlockBufs& last = p.blk.back();
   // d(low) = upsample^T(dy) [+ the gradient the fused loss scattered straight into the low-resolution map]
@@ -593,7 +649,7 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   int cur = 0;   // index of the scratch buffer holding d(block output)
   DDN_TRY(launch_fc_backward(c.f(p.dlow), p.tc ? nullptr : c.f(last.out), p.tc ? c.h(last.out_p.hi) : nullptr,
                              (p.tc && want_lo) ? c.h(last.out_p.lo) : nullptr, c.params + s.fc_w, S[cur], c.grads + s.fc_w,
-                             c.grads + s.fc_b, c.f(p.fc_part), (int64_t)h8 * w8, B, 512, p.D, c.st));
+                             c.grads + s.fc_b, c.f(p.fc_part), (int64_t)h8 * w8, B, s.fc_cin, p.D, c.st));
   std::vector<TcUnpackEntry> pending;      // tensor-core weight gradients waiting in dwp_all for the bucket's conversion
   auto defer = [&](const ConvSpec& cs) {
     if (!p.tc) return;
@@ -613,48 +669,58 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
     ++bucket_id; bucket_end = begin;
     return 0;
   };
-  bool b2_fused = false;    // the column sums of this block's bn2 came out of the next block's conv1 data gradient (slot 2)
+  bool out_fused = false;   // the column sums of this block's last BatchNorm came out of the next block's conv1 data gradient (slot 2)
   for (int i = (int)s.blocks.size() - 1; i >= 0; --i) {
     const BlockSpec& b = s.blocks[i]; const BlockBufs& bb = p.blk[i];
+    const int last = b.n - 1;
     const float* xin = p.tc ? nullptr : (i == 0 ? c.f(p.pool_out) : c.f(p.blk[i - 1].out));
     const PlaneBufs xin_p = i == 0 ? p.pool_p : p.blk[i - 1].out_p;
-    int64_t M1 = (int64_t)B * bb.c1.Hout * bb.c1.Wout;
+    auto rows = [&](const ConvBufs& cb) { return (int64_t)B * cb.Hout * cb.Wout; };
     int t1 = (cur + 1) & 3, t2 = (cur + 2) & 3, t3 = (cur + 3) & 3;
-    // out = relu(bn2(raw2) + residual):  g = dOut*(out>0) -> S[t2];  d raw2 -> planes (tensor core) or S[t1] (fp32)
-    DDN_TRY(bn_backward_for(c, b.b2, bb.c2, S[cur], p.tc ? nullptr : c.f(bb.out), p.tc ? c.h(bb.out_p.hi) : nullptr, 1, S[t2], b.c2,
-                            S[t1], M1, b2_fused ? 2 : 0));
-    // conv2: dW, d act1 -> S[t3] (+ the column sums of bn1's backward, in the same epilogue)
-    TcBwdStats st1, st2;
-    const bool b1_fused = bwd_stats_for(c, b.b1, bb.c1, nullptr, 1, &st1);
-    DDN_TRY(conv_backward(c, b.c2, p.tc ? nullptr : c.f(bb.act1), bb.act1_p, S[t1], S[t3], nullptr, B, bb.c2.Hin, bb.c2.Win, bb.c2.Hout,
-                          bb.c2.Wout, b.c2.cin, b1_fused ? &st1 : nullptr));
-    defer(b.c2);
-    // conv1's data gradient completes d(block input) = dOut of the previous block: bn2 of that block gets its column sums there
-    b2_fused = i > 0 && bwd_stats_for(c, s.blocks[i - 1].b2, p.blk[i - 1].c2, c.h(p.blk[i - 1].out_p.hi), 2, &st2);
-    // act1 = relu(bn1(raw1)), no residual: the mask is recomputed from raw1 in the tensor-core modes
+    // out = relu(bn_last(raw_last) + residual):  g = dOut*(out>0) -> S[t2];  d raw_last -> planes (tensor core) or S[t1] (fp32)
+    DDN_TRY(bn_backward_for(c, b.b[last], bb.c[last], S[cur], p.tc ? nullptr : c.f(bb.out), p.tc ? c.h(bb.out_p.hi) : nullptr, 1, S[t2],
+                            b.c[last], S[t1], rows(bb.c[last]), out_fused ? 2 : 0));
+    // conv_j (j = last .. 1): dW, d act[j-1] -> S[t3] (+ the column sums of bn_{j-1}'s backward, in the same epilogue); then
+    // act[j-1] = relu(bn_{j-1}(raw)), no residual: the mask is recomputed from raw in the tensor-core modes
+    TcBwdStats st_in, st_next;
+    bool in_fused = false;
+    for (int j = last; j >= 1; --j) {
+      in_fused = bwd_stats_for(c, b.b[j - 1], bb.c[j - 1], nullptr, 1, &st_in);
+      DDN_TRY(conv_backward(c, b.c[j], p.tc ? nullptr : c.f(bb.act[j - 1]), bb.act_p[j - 1], S[t1], S[t3], nullptr, B, bb.c[j].Hin,
+                            bb.c[j].Win, bb.c[j].Hout, bb.c[j].Wout, b.c[j].cin, in_fused ? &st_in : nullptr));
+      defer(b.c[j]);
+      if (j > 1)
+        DDN_TRY(bn_backward_for(c, b.b[j - 1], bb.c[j - 1], S[t3], p.tc ? nullptr : c.f(bb.act[j - 1]), nullptr, 1, nullptr, b.c[j - 1],
+                                S[t1], rows(bb.c[j - 1]), in_fused ? 1 : 0));
+    }
+    // conv1's data gradient completes d(block input) = dOut of the previous block: that block's last BatchNorm gets its column
+    // sums there
+    out_fused = i > 0 && bwd_stats_for(c, s.blocks[i - 1].b[last], p.blk[i - 1].c[last], c.h(p.blk[i - 1].out_p.hi), 2, &st_next);
     if (!b.has_ds) {
-      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, S[t1], M1,
-                              b1_fused ? 1 : 0));
+      DDN_TRY(bn_backward_for(c, b.b[0], bb.c[0], S[t3], p.tc ? nullptr : c.f(bb.act[0]), nullptr, 1, nullptr, b.c[0], S[t1],
+                              rows(bb.c[0]), in_fused ? 1 : 0));
       // dX = dgrad(conv1) + g
-      DDN_TRY(conv_backward(c, b.c1, xin, xin_p, S[t1], S[t3], S[t2], B, bb.c1.Hin, bb.c1.Win, bb.c1.Hout, bb.c1.Wout, b.c1.cin,
-                            b2_fused ? &st2 : nullptr));
-      defer(b.c1);
+      DDN_TRY(conv_backward(c, b.c[0], xin, xin_p, S[t1], S[t3], S[t2], B, bb.c[0].Hin, bb.c[0].Win, bb.c[0].Hout, bb.c[0].Wout, b.c[0].cin,
+                            out_fused ? &st_next : nullptr));
+      defer(b.c[0]);
       cur = t3;
     } else {
       // residual branch first (its dY planes are consumed before conv1's overwrite them):
       // bn_d(raw_d): d raw_d; ds conv: dW, dX_ds -> S[cur]
-      DDN_TRY(bn_backward_for(c, b.bd, bb.ds, S[t2], nullptr, nullptr, 0, nullptr, b.ds, S[t1], M1));
+      DDN_TRY(bn_backward_for(c, b.bd, bb.ds, S[t2], nullptr, nullptr, 0, nullptr, b.ds, S[t1], rows(bb.ds)));
       DDN_TRY(conv_backward(c, b.ds, xin, xin_p, S[t1], S[cur], nullptr, B, bb.ds.Hin, bb.ds.Win, bb.ds.Hout, bb.ds.Wout, b.ds.cin));
       defer(b.ds);
       // main branch: d raw1, then dX = dgrad(conv1) + dX_ds -> S[t2]
-      DDN_TRY(bn_backward_for(c, b.b1, bb.c1, S[t3], p.tc ? nullptr : c.f(bb.act1), nullptr, 1, nullptr, b.c1, S[t1], M1,
-                              b1_fused ? 1 : 0));
-      DDN_TRY(conv_backward(c, b.c1, xin, xin_p, S[t1], S[t2], S[cur], B, bb.c1.Hin, bb.c1.Win, bb.c1.Hout, bb.c1.Wout, b.c1.cin,
-                            b2_fused ? &st2 : nullptr));
-      defer(b.c1);
+      DDN_TRY(bn_backward_for(c, b.b[0], bb.c[0], S[t3], p.tc ? nullptr : c.f(bb.act[0]), nullptr, 1, nullptr, b.c[0], S[t1],
+                              rows(bb.c[0]), in_fused ? 1 : 0));
+      DDN_TRY(conv_backward(c, b.c[0], xin, xin_p, S[t1], S[t2], S[cur], B, bb.c[0].Hin, bb.c[0].Win, bb.c[0].Hout, bb.c[0].Wout, b.c[0].cin,
+                            out_fused ? &st_next : nullptr));
+      defer(b.c[0]);
       cur = t2;
       // a block with a downsample branch opens a residual layer: everything from its first parameter up is final now
-      DDN_TRY(close_bucket(b.c1.w_off));     // layer4 (+fc), layer3, layer2; layer1 + stem close at the end
+      // (layer4 (+fc), layer3, layer2; layer1 -- whose first block has a downsample in the Bottleneck network -- and the stem
+      // close together at the end)
+      if (i > 0) DDN_TRY(close_bucket(b.c[0].w_off));
     }
   }
   // stem: maxpool -> relu -> bn1 -> conv1 (weight gradient only; the image is not differentiated)
@@ -724,24 +790,103 @@ extern "C" int ddn_profile_read(ddn_profile_entry* out, int cap) {
   return k;
 }
 
-extern "C" int ddn_resnet34_8s_param_table(int D, ddn_tensor_entry* out, int cap) {
-  if (D < 1 || D > 32) return DDN_EINVAL;
-  const NetSpec& s = get_spec(D);
+static bool d_ok(int D) { return D >= 1 && D <= 32; }
+
+extern "C" int ddn_net_param_table(int arch, int D, ddn_tensor_entry* out, int cap) {
+  if (!arch_ok(arch) || !d_ok(D)) return DDN_EINVAL;
+  const NetSpec& s = get_spec(arch, D);
   for (int i = 0; i < (int)s.ptab.size() && i < cap && out; ++i) out[i] = s.ptab[i];
   return (int)s.ptab.size();
 }
-extern "C" int ddn_resnet34_8s_buffer_table(ddn_tensor_entry* out, int cap) {
-  const NetSpec& s = get_spec(3);
+extern "C" int ddn_net_buffer_table(int arch, ddn_tensor_entry* out, int cap) {
+  if (!arch_ok(arch)) return DDN_EINVAL;
+  const NetSpec& s = get_spec(arch, 3);
   for (int i = 0; i < (int)s.btab.size() && i < cap && out; ++i) out[i] = s.btab[i];
   return (int)s.btab.size();
 }
-extern "C" int64_t ddn_resnet34_8s_param_count(int D) { return (D < 1 || D > 32) ? DDN_EINVAL : get_spec(D).n_params; }
-extern "C" int64_t ddn_resnet34_8s_buffer_count(void) { return get_spec(3).n_buffers; }
-
-extern "C" size_t ddn_resnet34_8s_weight_cache_bytes(int D) {
-  if (D < 1 || D > 32) return 0;
-  return (size_t)get_spec(D).n_params * 2 * 2 * sizeof(__nv_bfloat16) + 4096;
+extern "C" int64_t ddn_net_param_count(int arch, int D) { return (!arch_ok(arch) || !d_ok(D)) ? DDN_EINVAL : get_spec(arch, D).n_params; }
+extern "C" int64_t ddn_net_buffer_count(int arch) { return arch_ok(arch) ? get_spec(arch, 3).n_buffers : DDN_EINVAL; }
+extern "C" size_t ddn_net_weight_cache_bytes(int arch, int D) {
+  if (!arch_ok(arch) || !d_ok(D)) return 0;
+  return (size_t)get_spec(arch, D).n_params * 2 * 2 * sizeof(__nv_bfloat16) + 4096;
 }
+extern "C" size_t ddn_net_workspace_bytes(int arch, int B, int H, int W, int D, int mode, int precision) {
+  Plan p;
+  if (make_plan(&p, arch, B, H, W, D, mode, precision) != 0) return 0;
+  return p.total;
+}
+
+static int check_ws(const Plan& p, void* ws, size_t bytes) {
+  DDN_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255) == 0, "workspace must be non-null and 256-byte aligned");
+  if (bytes < p.total) { set_error("workspace too small: %zu < %zu", bytes, p.total); return DDN_EWORKSPACE; }
+  return 0;
+}
+static int check_groups(int B, int G) {
+  DDN_CHECK_ARG(G >= 1 && G <= BN_MAX_GROUPS && B % G == 0, "bn_groups must be 1 or %d and divide the batch (got %d for B=%d)", BN_MAX_GROUPS, G, B);
+  return 0;
+}
+
+extern "C" int ddn_net_forward(int arch, const float* x, const float* params, float* buffers, float* y,
+                               void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                               int mode, int bn_groups, float momentum, float eps, int precision, float* low_nhwc_out,
+                               void* stream) {
+  DDN_CHECK_ARG(x && params && buffers && y, "null tensor");
+  DDN_TRY(check_groups(B, bn_groups));
+  Plan p;
+  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision));
+  DDN_TRY(check_ws(p, workspace, workspace_bytes));
+  Ctx c = {&get_spec(arch, D), &p, (char*)workspace, params, buffers, nullptr, (cudaStream_t)stream, momentum, eps, mode, bn_groups};
+  return net_forward(c, x, y, low_nhwc_out);
+}
+
+extern "C" int ddn_net_backward(int arch, const float* dy, const float* dlow_nhwc, const float* params, float* grads,
+                                void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                                int mode, int bn_groups, float eps, int precision,
+                                ddn_grad_bucket_fn on_bucket, void* user, void* stream) {
+  DDN_CHECK_ARG((dy || dlow_nhwc) && params && grads, "null tensor");
+  DDN_CHECK_ARG(mode == DDN_MODE_TRAIN || mode == DDN_MODE_EVAL_SAVE, "backward needs a forward that kept its activations (mode %d)", mode);
+  DDN_TRY(check_groups(B, bn_groups));
+  Plan p;
+  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision));
+  DDN_TRY(check_ws(p, workspace, workspace_bytes));
+  Ctx c = {&get_spec(arch, D), &p, (char*)workspace, params, nullptr, grads, (cudaStream_t)stream, 0.f, eps, mode, bn_groups};
+  return net_backward(c, dy, dlow_nhwc, on_bucket, user);
+}
+
+// layer4 + fc, layer3, layer2, then layer1 + stem (net_backward's close_bucket calls)
+extern "C" int ddn_net_grad_buckets(int arch, int D, int64_t* offsets, int cap) {
+  if (!arch_ok(arch) || !d_ok(D)) return DDN_EINVAL;
+  const NetSpec& s = get_spec(arch, D);
+  const int64_t b[5] = {s.blocks[s.layer_first[3]].c[0].w_off, s.blocks[s.layer_first[2]].c[0].w_off, s.blocks[s.layer_first[1]].c[0].w_off,
+                        0, s.n_params};
+  for (int i = 0; i < 5 && i < cap && offsets; ++i) offsets[i] = b[i];
+  return 4;
+}
+
+// ---- Resnet34_8s names of the entry points above
+extern "C" int ddn_resnet34_8s_param_table(int D, ddn_tensor_entry* out, int cap) { return ddn_net_param_table(DDN_ARCH_RESNET34_8S, D, out, cap); }
+extern "C" int ddn_resnet34_8s_buffer_table(ddn_tensor_entry* out, int cap) { return ddn_net_buffer_table(DDN_ARCH_RESNET34_8S, out, cap); }
+extern "C" int64_t ddn_resnet34_8s_param_count(int D) { return ddn_net_param_count(DDN_ARCH_RESNET34_8S, D); }
+extern "C" int64_t ddn_resnet34_8s_buffer_count(void) { return ddn_net_buffer_count(DDN_ARCH_RESNET34_8S); }
+extern "C" size_t ddn_resnet34_8s_weight_cache_bytes(int D) { return ddn_net_weight_cache_bytes(DDN_ARCH_RESNET34_8S, D); }
+extern "C" size_t ddn_resnet34_8s_workspace_bytes(int B, int H, int W, int D, int mode, int precision) {
+  return ddn_net_workspace_bytes(DDN_ARCH_RESNET34_8S, B, H, W, D, mode, precision);
+}
+extern "C" int ddn_resnet34_8s_forward(const float* x, const float* params, float* buffers, float* y,
+                                       void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                                       int mode, int bn_groups, float momentum, float eps, int precision, float* low_nhwc_out,
+                                       void* stream) {
+  return ddn_net_forward(DDN_ARCH_RESNET34_8S, x, params, buffers, y, workspace, workspace_bytes, B, H, W, D, mode, bn_groups, momentum, eps,
+                         precision, low_nhwc_out, stream);
+}
+extern "C" int ddn_resnet34_8s_backward(const float* dy, const float* dlow_nhwc, const float* params, float* grads,
+                                        void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                                        int mode, int bn_groups, float eps, int precision,
+                                        ddn_grad_bucket_fn on_bucket, void* user, void* stream) {
+  return ddn_net_backward(DDN_ARCH_RESNET34_8S, dy, dlow_nhwc, params, grads, workspace, workspace_bytes, B, H, W, D, mode, bn_groups, eps,
+                          precision, on_bucket, user, stream);
+}
+extern "C" int ddn_resnet34_8s_grad_buckets(int D, int64_t* offsets, int cap) { return ddn_net_grad_buckets(DDN_ARCH_RESNET34_8S, D, offsets, cap); }
 
 extern "C" int ddn_resnet34_8s_set_weight_cache(void* cache, size_t bytes, const float* params, uint64_t version, int precision) {
   std::lock_guard<std::mutex> lk(g_wcache_mu);
@@ -764,57 +909,6 @@ extern "C" int ddn_resnet34_8s_set_weight_cache(void* cache, size_t bytes, const
   }
   if (!cache) wc->params = nullptr;
   return 0;
-}
-
-extern "C" size_t ddn_resnet34_8s_workspace_bytes(int B, int H, int W, int D, int mode, int precision) {
-  Plan p;
-  if (make_plan(&p, B, H, W, D, mode, precision) != 0) return 0;
-  return p.total;
-}
-
-static int check_ws(const Plan& p, void* ws, size_t bytes) {
-  DDN_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255) == 0, "workspace must be non-null and 256-byte aligned");
-  if (bytes < p.total) { set_error("workspace too small: %zu < %zu", bytes, p.total); return DDN_EWORKSPACE; }
-  return 0;
-}
-static int check_groups(int B, int G) {
-  DDN_CHECK_ARG(G >= 1 && G <= BN_MAX_GROUPS && B % G == 0, "bn_groups must be 1 or %d and divide the batch (got %d for B=%d)", BN_MAX_GROUPS, G, B);
-  return 0;
-}
-
-extern "C" int ddn_resnet34_8s_forward(const float* x, const float* params, float* buffers, float* y,
-                                       void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
-                                       int mode, int bn_groups, float momentum, float eps, int precision, float* low_nhwc_out,
-                                       void* stream) {
-  DDN_CHECK_ARG(x && params && buffers && y, "null tensor");
-  DDN_TRY(check_groups(B, bn_groups));
-  Plan p;
-  DDN_TRY(make_plan(&p, B, H, W, D, mode, precision));
-  DDN_TRY(check_ws(p, workspace, workspace_bytes));
-  Ctx c = {&get_spec(D), &p, (char*)workspace, params, buffers, nullptr, (cudaStream_t)stream, momentum, eps, mode, bn_groups};
-  return net_forward(c, x, y, low_nhwc_out);
-}
-
-extern "C" int ddn_resnet34_8s_backward(const float* dy, const float* dlow_nhwc, const float* params, float* grads,
-                                        void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
-                                        int mode, int bn_groups, float eps, int precision,
-                                        ddn_grad_bucket_fn on_bucket, void* user, void* stream) {
-  DDN_CHECK_ARG((dy || dlow_nhwc) && params && grads, "null tensor");
-  DDN_CHECK_ARG(mode == DDN_MODE_TRAIN || mode == DDN_MODE_EVAL_SAVE, "backward needs a forward that kept its activations (mode %d)", mode);
-  DDN_TRY(check_groups(B, bn_groups));
-  Plan p;
-  DDN_TRY(make_plan(&p, B, H, W, D, mode, precision));
-  DDN_TRY(check_ws(p, workspace, workspace_bytes));
-  Ctx c = {&get_spec(D), &p, (char*)workspace, params, nullptr, grads, (cudaStream_t)stream, 0.f, eps, mode, bn_groups};
-  return net_backward(c, dy, dlow_nhwc, on_bucket, user);
-}
-
-extern "C" int ddn_resnet34_8s_grad_buckets(int D, int64_t* offsets, int cap) {
-  if (D < 1 || D > 32) return DDN_EINVAL;
-  const NetSpec& s = get_spec(D);
-  const int64_t b[5] = {s.blocks[13].c1.w_off, s.blocks[7].c1.w_off, s.blocks[3].c1.w_off, 0, s.n_params};
-  for (int i = 0; i < 5 && i < cap && offsets; ++i) offsets[i] = b[i];
-  return 4;
 }
 
 // ------------------------------------------------------------------------------------------------ single operators

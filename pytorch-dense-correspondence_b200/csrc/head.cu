@@ -351,10 +351,199 @@ fc_wgrad_planes_kernel(const float* __restrict__ dlow, const __nv_bfloat16* __re
   }
 }
 
+// ---- the same three for a wide trunk (C > 512: the 2048 channels of the Bottleneck backbone).  [D][C] fp32 weights no longer
+// fit in shared memory (256 KB at D = 32, C = 2048) and one partial slot of the weight gradient holds D*C floats, so every kernel
+// below walks the channels in chunks of FC_WIDE_CHUNK, and the weight gradient keeps FC_WIDE_SLOTS pixel slots.
+constexpr int FC_WIDE_CHUNK = 512;
+constexpr int FC_WIDE_TILE = 64;        // pixels per forward tile: 8 warps x 8 pixels
+constexpr int FC_WIDE_SLOTS = 64;
+constexpr int FC_WIDE_WG_CH = 256;      // channels of one weight-gradient block: 64 threads x 4 channels
+
+// low[n][d][p] = bias[d] + sum_c feat[n][p][c] * w[d][c]: per tile of 64 pixels, the chunk's weights are staged in shared memory
+// and every warp adds the chunk's dot products of its pixels to the tile's accumulators (fixed chunk order: deterministic)
+template <int DM>
+__global__ void __launch_bounds__(256)
+fc_forward_wide_kernel(const float* __restrict__ feat, const __nv_bfloat16* __restrict__ feat_hi, const __nv_bfloat16* __restrict__ feat_lo,
+                       const float* __restrict__ w, const float* __restrict__ bias,
+                       float* __restrict__ low, float* __restrict__ low_t, int64_t Mimg, int N, int C, int D) {
+  pdl_prologue();
+  extern __shared__ float sm[];           // [D][FC_WIDE_CHUNK] weights, then [FC_WIDE_TILE][D] accumulators
+  float* ws = sm;
+  float* acc_s = sm + D * FC_WIDE_CHUNK;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t total = (int64_t)N * Mimg;
+  const int64_t n_tiles = (total + FC_WIDE_TILE - 1) / FC_WIDE_TILE;
+  const int q = C >> 2;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t pix0 = tile * FC_WIDE_TILE;
+    for (int c0 = 0; c0 < C; c0 += FC_WIDE_CHUNK) {
+      __syncthreads();                    // the previous chunk's weights are no longer read
+      for (int i = threadIdx.x; i < D * FC_WIDE_CHUNK; i += blockDim.x) {
+        const int d = i / FC_WIDE_CHUNK, j = i - d * FC_WIDE_CHUNK;
+        ws[i] = w[(size_t)d * C + c0 + j];
+      }
+      __syncthreads();
+      for (int pl = warp; pl < FC_WIDE_TILE; pl += 8) {
+        const int64_t pix = pix0 + pl;
+        if (pix >= total) break;
+        float acc[DM];
+#pragma unroll
+        for (int d = 0; d < DM; ++d) acc[d] = 0.f;
+        for (int c4 = lane; c4 < FC_WIDE_CHUNK / 4; c4 += 32) {
+          const float4 v = load_feat4(feat, feat_hi, feat_lo, pix * q + (c0 >> 2) + c4);
+#pragma unroll
+          for (int d = 0; d < DM; ++d) {
+            if (d < D) {
+              const float4 wv = *reinterpret_cast<const float4*>(ws + d * FC_WIDE_CHUNK + (c4 << 2));
+              acc[d] = fmaf(v.x, wv.x, fmaf(v.y, wv.y, fmaf(v.z, wv.z, fmaf(v.w, wv.w, acc[d]))));
+            }
+          }
+        }
+#pragma unroll
+        for (int d = 0; d < DM; ++d) {
+          if (d < D) {
+            const float t = warp_sum(acc[d]);
+            if (lane == 0) acc_s[pl * D + d] = c0 == 0 ? t : acc_s[pl * D + d] + t;
+          }
+        }
+      }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < FC_WIDE_TILE * D; i += blockDim.x) {
+      const int pl = i / D, d = i - pl * D;
+      const int64_t pix = pix0 + pl;
+      if (pix >= total) continue;
+      const int64_t n = pix / Mimg, p = pix - n * Mimg;
+      const float v = acc_s[i] + bias[d];
+      low[(n * D + d) * Mimg + p] = v;
+      if (low_t) low_t[pix * D + d] = v;
+    }
+  }
+}
+
+// dfeat[n][p][c] = sum_d dlow[n][d][p] * w[d][c]; blockIdx.y = channel chunk, its [D][FC_WIDE_CHUNK] weights in shared memory
+template <int DM>
+__global__ void __launch_bounds__(256)
+fc_dgrad_wide_kernel(const float* __restrict__ dlow, const float* __restrict__ w, float* __restrict__ dfeat, int64_t Mimg, int N, int C, int D) {
+  pdl_prologue();
+  extern __shared__ float ws[];
+  const int c0 = blockIdx.y * FC_WIDE_CHUNK;
+  for (int i = threadIdx.x; i < D * FC_WIDE_CHUNK; i += blockDim.x) {
+    const int d = i / FC_WIDE_CHUNK, j = i - d * FC_WIDE_CHUNK;
+    ws[i] = w[(size_t)d * C + c0 + j];
+  }
+  __syncthreads();
+  constexpr int QC = FC_WIDE_CHUNK / 4;
+  const int64_t total = (int64_t)N * Mimg * QC;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int cl = (int)(i % QC) << 2; const int64_t pix = i / QC;
+    const int64_t n = pix / Mimg, p = pix - n * Mimg;
+    float4 a = make_float4(0, 0, 0, 0);
+#pragma unroll
+    for (int d = 0; d < DM; ++d) {
+      if (d < D) {
+        const float g = __ldg(dlow + (n * D + d) * Mimg + p);
+        const float4 wv = *reinterpret_cast<const float4*>(ws + d * FC_WIDE_CHUNK + cl);
+        a.x = fmaf(g, wv.x, a.x); a.y = fmaf(g, wv.y, a.y); a.z = fmaf(g, wv.z, a.z); a.w = fmaf(g, wv.w, a.w);
+      }
+    }
+    reinterpret_cast<float4*>(dfeat + pix * C + c0)[cl >> 2] = a;
+  }
+}
+
+// dw[d][c] / dbias[d] partial sums: blockIdx.x = pixel slot (a contiguous pixel range), blockIdx.y = 256-channel chunk.  Thread =
+// 4 consecutive channels (one 8-byte load per plane and pixel) x one of 4 pixel rows; the rows are folded through shared memory
+// in a fixed order and the block writes its chunk of slot blockIdx.x.  fc_part_reduce_kernel adds the slots in slot order.
+template <int DM>
+__global__ void __launch_bounds__(256)
+fc_wgrad_wide_kernel(const float* __restrict__ dlow, const float* __restrict__ feat, const __nv_bfloat16* __restrict__ feat_hi,
+                     const __nv_bfloat16* __restrict__ feat_lo, float* __restrict__ part, int64_t Mimg, int N, int C, int D, int pix_per_slot) {
+  pdl_prologue();
+  const int64_t total = (int64_t)N * Mimg;
+  const int64_t p0 = (int64_t)blockIdx.x * pix_per_slot;
+  const int64_t p1 = min(total, p0 + pix_per_slot);
+  const int cq = threadIdx.x & 63, rr = threadIdx.x >> 6;
+  const int c = blockIdx.y * FC_WIDE_WG_CH + cq * 4;
+  float acc[4][DM];
+  float bsum[DM];
+#pragma unroll
+  for (int d = 0; d < DM; ++d) {
+    bsum[d] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[j][d] = 0.f;
+  }
+  for (int64_t pix = p0 + rr; pix < p1; pix += 4) {
+    const float4 f = load_feat4(feat, feat_hi, feat_lo, (pix * C + c) >> 2);
+    const int64_t n = pix / Mimg, p = pix - n * Mimg;
+#pragma unroll
+    for (int d = 0; d < DM; ++d) {
+      const float g = d < D ? __ldg(dlow + (n * D + d) * Mimg + p) : 0.f;
+      acc[0][d] = fmaf(g, f.x, acc[0][d]); acc[1][d] = fmaf(g, f.y, acc[1][d]);
+      acc[2][d] = fmaf(g, f.z, acc[2][d]); acc[3][d] = fmaf(g, f.w, acc[3][d]);
+      bsum[d] += g;
+    }
+  }
+  __shared__ float s_acc[DM][FC_WIDE_WG_CH];
+  __shared__ float s_b[4][DM];
+  if (cq == 0) {
+#pragma unroll
+    for (int d = 0; d < DM; ++d) s_b[rr][d] = bsum[d];
+  }
+  for (int r = 1; r < 4; ++r) {
+    if (rr == r) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int d = 0; d < DM; ++d) s_acc[d][cq * 4 + j] = acc[j][d];
+    }
+    __syncthreads();
+    if (rr == 0) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int d = 0; d < DM; ++d) acc[j][d] += s_acc[d][cq * 4 + j];
+    }
+    __syncthreads();
+  }
+  if (rr == 0) {
+    float* slot = part + (size_t)blockIdx.x * (D * C + D);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int d = 0; d < DM; ++d)
+        if (d < D) slot[d * C + c + j] = acc[j][d];
+    if (cq == 0 && blockIdx.y == 0) {
+#pragma unroll
+      for (int d = 0; d < DM; ++d)
+        if (d < D) slot[D * C + d] = s_b[0][d] + s_b[1][d] + s_b[2][d] + s_b[3][d];
+    }
+  }
+}
+
+size_t fc_part_floats(int C, int D) {
+  return C <= 512 ? (size_t)FC_PART_SLOTS * (D * C + D) : (size_t)FC_WIDE_SLOTS * (D * C + D);
+}
+
+static int check_fc(const float* feat, const __nv_bfloat16* feat_hi, int C, int D) {
+  DDN_CHECK_ARG(feat || feat_hi, "fc: no feature tensor");
+  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD && C % 4 == 0 && (C <= 512 || C % FC_WIDE_CHUNK == 0),
+                "fc: need 1<=D<=32 and C%%4==0 with C<=512 or C a multiple of %d (got C=%d D=%d)", FC_WIDE_CHUNK, C, D);
+  return 0;
+}
+
 int launch_fc_forward(const float* feat, const __nv_bfloat16* feat_hi, const __nv_bfloat16* feat_lo, const float* w, const float* bias,
                       float* low, float* low_nhwc, int64_t Mimg, int N, int C, int D, cudaStream_t st) {
-  DDN_CHECK_ARG(feat || feat_hi, "fc: no feature tensor");
-  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD && C % 4 == 0 && C <= 512, "fc: need 1<=D<=32, C%%4==0, C<=512");
+  DDN_TRY(check_fc(feat, feat_hi, C, D));
+  if (C > 512) {
+    const size_t smem = sizeof(float) * ((size_t)D * FC_WIDE_CHUNK + (size_t)FC_WIDE_TILE * D);
+    const int blocks = (int)std::min<int64_t>(ceil_div((int64_t)N * Mimg, FC_WIDE_TILE), (int64_t)num_sms() * 4);
+#define CALL(DM)                                                                                                       \
+  DDN_CUDA(cudaFuncSetAttribute(fc_forward_wide_kernel<DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
+  DDN_LAUNCH(fc_forward_wide_kernel<DM>, blocks, 256, smem, st, feat, feat_hi, feat_lo, w, bias, low, low_nhwc, Mimg, N, C, D)
+    FC_DISPATCH(D, CALL);
+#undef CALL
+    return 0;
+  }
   size_t smem = sizeof(float) * D * C;
   int blocks = (int)std::min<int64_t>(ceil_div((int64_t)N * Mimg, 8), (int64_t)num_sms() * 8);
 #define CALL(DM)                                                                                              \
@@ -367,8 +556,28 @@ int launch_fc_forward(const float* feat, const __nv_bfloat16* feat_hi, const __n
 
 int launch_fc_backward(const float* dlow, const float* feat, const __nv_bfloat16* feat_hi, const __nv_bfloat16* feat_lo, const float* w,
                        float* dfeat, float* dw, float* dbias, float* part, int64_t Mimg, int N, int C, int D, cudaStream_t st) {
-  DDN_CHECK_ARG(feat || feat_hi, "fc: no feature tensor");
-  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD && C % 4 == 0 && C <= 512, "fc: need 1<=D<=32, C%%4==0, C<=512");
+  DDN_TRY(check_fc(feat, feat_hi, C, D));
+  if (C > 512) {
+    const int64_t total = (int64_t)N * Mimg;
+    const size_t smem = sizeof(float) * (size_t)D * FC_WIDE_CHUNK;
+    const int chunks = C / FC_WIDE_CHUNK;
+    dim3 dgrid((unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(total * (FC_WIDE_CHUNK / 4), 256), (int64_t)num_sms() * 8 / chunks)),
+               (unsigned)chunks);
+#define CALL(DM)                                                                                                    \
+  DDN_CUDA(cudaFuncSetAttribute(fc_dgrad_wide_kernel<DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
+  DDN_LAUNCH(fc_dgrad_wide_kernel<DM>, dgrid, 256, smem, st, dlow, w, dfeat, Mimg, N, C, D)
+    FC_DISPATCH(D, CALL);
+#undef CALL
+    const int pps = (int)ceil_div(total, FC_WIDE_SLOTS);
+    const int slots = (int)ceil_div(total, pps);           // <= FC_WIDE_SLOTS
+    dim3 wgrid((unsigned)slots, (unsigned)(C / FC_WIDE_WG_CH));
+#define CALL(DM) DDN_LAUNCH(fc_wgrad_wide_kernel<DM>, wgrid, 256, 0, st, dlow, feat, feat_hi, feat_lo, part, Mimg, N, C, D, pps)
+    FC_DISPATCH(D, CALL);
+#undef CALL
+    const int slot_len = D * C + D;
+    DDN_LAUNCH(fc_part_reduce_kernel, (int)ceil_div(slot_len, 256), 256, 0, st, part, slots, slot_len, D * C, dw, dbias);
+    return 0;
+  }
   size_t smem = sizeof(float) * D * C;
   int64_t total = (int64_t)N * Mimg;
 #define CALL(DM)                                                                                               \

@@ -161,11 +161,11 @@ class DenseCorrespondenceNetwork(nn.Module):
 
     @staticmethod
     def get_fcn(config):
-        """net.py:360-383.  Only Resnet34_8s exists in this build; anything else raises (no fallback)."""
+        """net.py:360-383.  Resnet34_8s and Resnet50_8s exist in this build; anything else raises (no fallback)."""
         if config["backbone"]["model_class"] == "Resnet":
             resnet_model = config["backbone"]["resnet_name"]
-            if not hasattr(resnet_dilated, resnet_model):
-                raise ValueError("backbone %s is not implemented in this path (only Resnet34_8s)" % resnet_model)
+            if resnet_model not in ("Resnet34_8s", "Resnet50_8s"):
+                raise ValueError("backbone %s is not implemented in this path (only Resnet34_8s and Resnet50_8s)" % resnet_model)
             fcn = getattr(resnet_dilated, resnet_model)(num_classes=config['descriptor_dimension'])
         elif config["backbone"]["model_class"] == "Unet":
             fcn = DenseCorrespondenceNetwork.get_unet(config)

@@ -1,8 +1,10 @@
-"""Resnet34_8s -- drop-in for the backbone class the reference builds with
-``getattr(resnet_dilated, "Resnet34_8s")(num_classes=D)``
+"""Resnet34_8s and Resnet50_8s -- drop-ins for the backbone classes the reference builds with
+``getattr(resnet_dilated, config["backbone"]["resnet_name"])(num_classes=D)``
 (dense_correspondence/network/dense_correspondence_network.py:373-375;
-original: external/pytorch-segmentation-detection/pytorch_segmentation_detection/models/resnet_dilated.py:283-322
-on top of .../vision/torchvision/models/resnet.py:112-265).
+originals: external/pytorch-segmentation-detection/pytorch_segmentation_detection/models/resnet_dilated.py:283-322 and
+:399-435 on top of .../vision/torchvision/models/resnet.py:112-265 -- BasicBlock [3, 4, 6, 3] and Bottleneck [3, 4, 6, 3]).
+The description below says Resnet34_8s; Resnet50_8s is the same module over its own parameter tables (``resnet50_8s.*``, 320
+state-dict keys).
 
 Same constructor, same ``forward(x, feature_alignment=False)``, same 218 state-dict keys
 (``resnet34_8s.conv1.weight`` ... ``resnet34_8s.fc.bias``), same train()/eval() BatchNorm semantics --
@@ -63,7 +65,7 @@ class _Holder(nn.Module):
     """A name-space node of the reference module tree (it owns parameters/buffers, never computes)."""
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("Resnet34_8s sub-modules are parameter holders; call the top-level module")
+        raise RuntimeError("backbone sub-modules are parameter holders; call the top-level module")
 
 
 class _Backbone(torch.autograd.Function):
@@ -95,16 +97,17 @@ class _Backbone(torch.autograd.Function):
         prec = owner.precision
         _check_precision(prec)
         owner._register_weight_cache(flat, prec)
-        ws_bytes = N.lib.ddn_resnet34_8s_workspace_bytes(B, H, W, D, mode, prec)
+        arch = owner._ARCH
+        ws_bytes = N.lib.ddn_net_workspace_bytes(arch, B, H, W, D, mode, prec)
         if ws_bytes == 0:
-            raise N.DdnError("bad shape for Resnet34_8s: %s" % N.lib.ddn_last_error().decode())
+            raise N.DdnError("bad shape for %s: %s" % (type(owner).__name__, N.lib.ddn_last_error().decode()))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
         y = torch.empty(B, D, H, W, dtype=torch.float32, device=x.device)
         # the low-resolution map y is the bilinear upsample of, [B, H/8*W/8, D]: second output, so that a loss fused with the
         # upsample (contrastive_ops.within_scene_loss on tensors carrying `_ddn_lowres`) can differentiate through it directly
         low = torch.empty(B, (H // 8) * (W // 8), D, dtype=torch.float32, device=x.device)
-        N.check(N.lib.ddn_resnet34_8s_forward(N.ptr(x), N.ptr(flat), N.ptr(bufs), N.ptr(y), N.ptr(ws), ws_bytes,
-                                              B, H, W, D, mode, groups, _BN_MOMENTUM, _BN_EPS, prec, N.ptr(low), N.stream_ptr()))
+        N.check(N.lib.ddn_net_forward(arch, N.ptr(x), N.ptr(flat), N.ptr(bufs), N.ptr(y), N.ptr(ws), ws_bytes,
+                                      B, H, W, D, mode, groups, _BN_MOMENTUM, _BN_EPS, prec, N.ptr(low), N.stream_ptr()))
         ctx.set_materialize_grads(False)
         if owner.training:
             torch._foreach_add_(owner._nbt, groups)
@@ -119,9 +122,9 @@ class _Backbone(torch.autograd.Function):
         if dy is None and dlow is None:
             return (None, None, None) + (None,) * len(ctx.owner._params) if ctx.keep else None
         if not ctx.keep:
-            raise RuntimeError("Resnet34_8s.backward: nothing required a gradient in the forward; no activations were saved")
+            raise RuntimeError("backbone backward: nothing required a gradient in the forward; no activations were saved")
         if ctx.ws is None:
-            raise RuntimeError("Resnet34_8s: trying to backward through the backbone a second time; its saved activations "
+            raise RuntimeError("backbone: trying to backward through the backbone a second time; its saved activations "
                                "(one caller-owned workspace) were released by the first backward -- retain_graph is not supported")
         owner = ctx.owner
         B, H, W, D = ctx.shape
@@ -149,8 +152,8 @@ class _Backbone(torch.autograd.Function):
             def _on_bucket(_user, bucket, offset, numel, _g=grads, _h=hook):
                 _h.__call_bucket__(_g, int(bucket), int(offset), int(numel))
             cb = N.GRAD_BUCKET_FN(_on_bucket)
-        N.check(N.lib.ddn_resnet34_8s_backward(N.ptr(dy), N.ptr(dlow), N.ptr(flat), N.ptr(grads), N.ptr(ctx.ws), ctx.ws.numel(),
-                                               B, H, W, D, ctx.mode, ctx.groups, _BN_EPS, ctx.prec, cb, None, N.stream_ptr()))
+        N.check(N.lib.ddn_net_backward(owner._ARCH, N.ptr(dy), N.ptr(dlow), N.ptr(flat), N.ptr(grads), N.ptr(ctx.ws), ctx.ws.numel(),
+                                       B, H, W, D, ctx.mode, ctx.groups, _BN_EPS, ctx.prec, cb, None, N.stream_ptr()))
         ctx.ws = None
         if hook is not None:
             hook.finish(grads)
@@ -183,7 +186,11 @@ class _Backbone(torch.autograd.Function):
         return (None, None, None) + (None,) * len(ps)
 
 
-class Resnet34_8s(nn.Module):
+class _DilatedResnet(nn.Module):
+    """The flat-array backbone; subclasses name the architecture (``_ARCH``) and the reference's root attribute (``_ROOT``)."""
+    _ARCH = None
+    _ROOT = None
+
     def _pad_index_on(self, device):
         t = self._pad_index_dev.get(device)
         if t is None:
@@ -196,10 +203,10 @@ class Resnet34_8s(nn.Module):
             raise ValueError("this build supports descriptor dimensions 1..32 (got %d)" % num_classes)
         self.num_classes = num_classes
         self.precision = _default_precision[0] if precision is None else precision
-        self._ptab = N.param_table(num_classes)
-        self._btab = N.buffer_table()
-        n_params = int(N.lib.ddn_resnet34_8s_param_count(num_classes))
-        n_bufs = int(N.lib.ddn_resnet34_8s_buffer_count())
+        self._ptab = N.param_table(num_classes, self._ARCH)
+        self._btab = N.buffer_table(self._ARCH)
+        n_params = int(N.lib.ddn_net_param_count(self._ARCH, num_classes))
+        n_bufs = int(N.lib.ddn_net_buffer_count(self._ARCH))
         self._flat = torch.zeros(n_params, dtype=torch.float32)
         self._flat_bufs = torch.zeros(n_bufs, dtype=torch.float32)
         self._flat_version = 0
@@ -215,7 +222,7 @@ class Resnet34_8s(nn.Module):
         self._params = []
         self._nbt = []
         root = _Holder()
-        self.resnet34_8s = root
+        setattr(self, self._ROOT, root)
         buf_by_name = {name: (shape, off, n) for name, shape, off, n in self._btab}
         for name, shape, off, n in self._ptab:
             path = name.split(".")
@@ -266,7 +273,7 @@ class Resnet34_8s(nn.Module):
             if m.running_mean.device != device:
                 return False
         for (name, _, off, _) in self._btab:
-            node = self.resnet34_8s
+            node = getattr(self, self._ROOT)
             parts = name.split(".")
             for part in parts[:-1]:
                 node = getattr(node, part)
@@ -286,7 +293,7 @@ class Resnet34_8s(nn.Module):
                 p.data = flat[off:off + n].view(shape)
             bufs = torch.zeros(self._flat_bufs.numel(), dtype=torch.float32, device=device)
             for (name, shape, off, n) in self._btab:
-                node = self.resnet34_8s
+                node = getattr(self, self._ROOT)
                 parts = name.split(".")
                 for part in parts[:-1]:
                     node = getattr(node, part)
@@ -317,7 +324,7 @@ class Resnet34_8s(nn.Module):
         if prec == N.PRECISION_FP32_SIMT:
             return
         if self._wcache is None or self._wcache.device != flat.device:
-            self._wcache = torch.empty(N.lib.ddn_resnet34_8s_weight_cache_bytes(self.num_classes), dtype=torch.uint8,
+            self._wcache = torch.empty(N.lib.ddn_net_weight_cache_bytes(self._ARCH, self.num_classes), dtype=torch.uint8,
                                        device=flat.device)
             _cache_nonce[0] += 1           # a fresh buffer may reuse the address of a dead one: never look "unchanged"
             self._wcache_nonce = _cache_nonce[0]
@@ -348,3 +355,15 @@ class Resnet34_8s(nn.Module):
         y, low = _Backbone.apply(x, self, bn_groups, *self._params)
         attach_lowres(y, low, x.shape[2], x.shape[3])
         return y
+
+
+class Resnet34_8s(_DilatedResnet):
+    """resnet_dilated.py:283-322: ResNet(BasicBlock, [3, 4, 6, 3]), output stride 8, fc = Conv2d(512, D, 1)."""
+    _ARCH = N.ARCH_RESNET34_8S
+    _ROOT = "resnet34_8s"
+
+
+class Resnet50_8s(_DilatedResnet):
+    """resnet_dilated.py:399-435: ResNet(Bottleneck, [3, 4, 6, 3]), output stride 8, fc = Conv2d(2048, D, 1)."""
+    _ARCH = N.ARCH_RESNET50_8S
+    _ROOT = "resnet50_8s"
