@@ -78,9 +78,8 @@ int launch_nchw_to_nhwc4(const float* x, float* y, int N, int H, int W, cudaStre
 int launch_fc_forward(const float* feat, const __nv_bfloat16* feat_hi, const __nv_bfloat16* feat_lo, const float* w, const float* bias,
                       float* low, float* low_nhwc, int64_t Mimg, int N, int C, int D, cudaStream_t st);
 int launch_add_lowres_nhwc(const float* dlow_nhwc, float* dlow, int64_t Mimg, int N, int D, int accumulate, cudaStream_t st);
-// part: FC_PART_SLOTS * (D * C + D) floats of scratch (per-block partial sums of dw / dbias, added in a fixed order)
-constexpr int FC_PART_SLOTS = 512;
-size_t fc_part_floats(int C, int D);      // the `part` scratch launch_fc_backward needs for C channels (C > 512: fewer, wider slots)
+// part: fc_part_floats(C, D) floats of scratch (per-slot partial sums of dw / dbias, added in a fixed order)
+size_t fc_part_floats(int C, int D);
 int launch_fc_backward(const float* dlow, const float* feat, const __nv_bfloat16* feat_hi, const __nv_bfloat16* feat_lo, const float* w,
                        float* dfeat, float* dw, float* dbias, float* part, int64_t Mimg, int N, int C, int D, cudaStream_t st);
 int launch_upsample_fwd(const float* x, float* y, int NC, int h, int w, int H, int W, cudaStream_t st);
