@@ -287,6 +287,7 @@ int ddn_batchnorm_backward(const float* dy, const float* x, const float* y, cons
                            const float* save_mean, const float* save_invstd,
                            float* dx, float* dgamma, float* dbeta, float* d_residual,
                            int64_t M, int C, int relu, void* workspace, size_t workspace_bytes, void* stream);
+/* 0 for a C the BatchNorm kernels do not take: they need 4 <= C <= 1024 with 256 % (C/4) == 0, or a multiple of 1024 up to 4096. */
 size_t ddn_batchnorm_workspace_bytes(int64_t M, int C);
 
 /* Tensor-core convolutions with the fused epilogues the network runs (resnet.py:53-69 conv -> BatchNorm -> [+ residual] -> ReLU),
@@ -328,6 +329,20 @@ int ddn_conv2d_backward_data_bn_stats(const float* w_oihw, const float* dy_nhwc,
  * (nn.functional.upsample_bilinear, resnet_dilated.py:320) and its adjoint. */
 int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, int h, int w, int H, int W, void* stream);
 int ddn_upsample_bilinear_backward(const float* dy, float* dx, int NC, int h, int w, int H, int W, void* stream);
+
+/* The scoring layer fc = nn.Conv2d(C, D, 1) with bias (resnet_dilated.py:298 for C = 512, :414 for C = 2048) on the trunk's
+ * channels-last features, and its backward.  feat [N*Mimg, C] fp32, or its bf16 operand planes (feat = hi + lo; feat_lo may be
+ * NULL: hi alone) -- exactly one of the two; w [D, C], bias [D]; low / dlow [N, D, Mimg] (the planar map the upsample reads);
+ * low_nhwc (optional) [N*Mimg, D].  1 <= D <= 32, C a multiple of 512; feat, feat_hi, feat_lo and dfeat 16-byte aligned.
+ * The backward overwrites dfeat [N*Mimg, C], dw [D, C] and dbias [D]; its workspace (ddn_fc_workspace_bytes, 0 for an
+ * unsupported C, D) holds per-slot partial sums that are added in a fixed order, so the result is the same on every run.
+ * Every argument is checked before anything is launched. */
+size_t ddn_fc_workspace_bytes(int C, int D);
+int ddn_fc_forward(const float* feat, const void* feat_hi_bf16, const void* feat_lo_bf16, const float* w, const float* bias,
+                   float* low, float* low_nhwc, int64_t Mimg, int N, int C, int D, void* stream);
+int ddn_fc_backward(const float* dlow, const float* feat, const void* feat_hi_bf16, const void* feat_lo_bf16, const float* w,
+                    float* dfeat, float* dw, float* dbias, int64_t Mimg, int N, int C, int D,
+                    void* workspace, size_t workspace_bytes, void* stream);
 
 /* Data-parallel helpers on the flat gradient: g *= scale (after an all-reduce SUM over ranks). */
 int ddn_scale_inplace(float* g, int64_t n, float scale, void* stream);

@@ -89,6 +89,9 @@ _SIGNATURES = {
     "ddn_batchnorm_backward": (i32, [vp] * 10 + [i64, i32, i32, vp, sz, vp]),
     "ddn_upsample_bilinear_forward": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
     "ddn_upsample_bilinear_backward": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+    "ddn_fc_workspace_bytes": (sz, [i32, i32]),
+    "ddn_fc_forward": (i32, [vp] * 7 + [i64, i32, i32, i32, vp]),
+    "ddn_fc_backward": (i32, [vp] * 8 + [i64, i32, i32, i32, vp, sz, vp]),
     "ddn_scale_inplace": (i32, [vp, i64, f32, vp]),
     "ddn_sample_non_matches_scratch_bytes": (sz, [i32, i32]),
     "ddn_sample_non_matches": (i32, [vp, i32, i32, vp, vp, i64, vp, i64, vp, vp, vp, sz, vp]),

@@ -403,9 +403,12 @@ stem_pool_relu_bwd_kernel(const float* __restrict__ dyp, const uint8_t* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ launchers
+bool bn_c_supported(int C) {
+  return C >= 4 && C % 4 == 0 && (C <= BN_COLSUM_MAX_C ? BN_THREADS % (C / 4) == 0 : (C % BN_COLSUM_MAX_C == 0 && C <= 4096));
+}
+
 static int check_c(int C, int G, int64_t M) {
-  DDN_CHECK_ARG(C >= 4 && C % 4 == 0 && (C <= BN_COLSUM_MAX_C ? BN_THREADS % (C / 4) == 0 : (C % BN_COLSUM_MAX_C == 0 && C <= 4096)),
-                "BatchNorm kernels need C in {4..1024} with 256 %% (C/4) == 0, or a multiple of 1024 up to 4096 (got %d)", C);
+  DDN_CHECK_ARG(bn_c_supported(C), "BatchNorm kernels need C in {4..1024} with 256 %% (C/4) == 0, or a multiple of 1024 up to 4096 (got %d)", C);
   DDN_CHECK_ARG(G >= 1 && G <= BN_MAX_GROUPS && M % G == 0, "BatchNorm groups: need 1 <= G <= %d dividing the row count", BN_MAX_GROUPS);
   return 0;
 }

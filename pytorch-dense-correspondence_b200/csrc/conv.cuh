@@ -24,6 +24,7 @@ int launch_conv_gather_f32(const float* in, const float* wp, const float* addend
 int launch_conv_wgrad_f32(const float* in, const float* dy, float* dwp, const ConvGeom& g, cudaStream_t st);
 
 // bn.cu -- NHWC tensors viewed as [M = N*H*W][C]; G BatchNorm groups of M/G consecutive rows each (bn_stats.cuh)
+bool bn_c_supported(int C);                       // the channel counts the BatchNorm kernels take
 size_t bn_accum_bytes(int C);                     // BnAccum storage for C channels (acc + ticket), zero-filled by the owner
 BnAccum bn_accum_at(void* base, int C);
 // column sums of x -> mean / invstd [G][C] (+ running statistics): one launch, finalized by the last CTA

@@ -971,7 +971,7 @@ extern "C" int ddn_conv2d_backward(const float* x, const float* w, const float* 
 
 extern "C" size_t ddn_batchnorm_workspace_bytes(int64_t M, int C) {
   (void)M;
-  if (C < 4 || C % 4 || 256 % (C / 4)) return 0;
+  if (!bn_c_supported(C)) return 0;
   return bn_accum_bytes(C) + sizeof(float) * 2 * BN_MAX_GROUPS * C + 256;
 }
 

@@ -352,10 +352,14 @@ static FcSlots fc_slots(int C) { return C <= 512 ? FcSlots{512, 16} : FcSlots{64
 
 size_t fc_part_floats(int C, int D) { return (size_t)fc_slots(C).max_slots * (D * C + D); }
 
+// the kernels index one slot of `part` (D*C + D floats) with int
+static bool fc_shape_ok(int C, int D) {
+  return D >= 1 && D <= FC_MAXD && C > 0 && C % FC_CHUNK == 0 && (int64_t)D * C + D <= INT32_MAX;
+}
+
 static int check_fc(const float* feat, const __nv_bfloat16* feat_hi, int C, int D) {
   DDN_CHECK_ARG(feat || feat_hi, "fc: no feature tensor");
-  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD && C > 0 && C % FC_CHUNK == 0,
-                "fc: need 1<=D<=32 and C a multiple of %d (got C=%d D=%d)", FC_CHUNK, C, D);
+  DDN_CHECK_ARG(fc_shape_ok(C, D), "fc: need 1<=D<=32 and C a multiple of %d (got C=%d D=%d)", FC_CHUNK, C, D);
   return 0;
 }
 
@@ -451,4 +455,38 @@ extern "C" int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, i
 extern "C" int ddn_upsample_bilinear_backward(const float* dy, float* dx, int NC, int h, int w, int H, int W, void* stream) {
   DDN_CHECK_ARG(dy && dx && NC > 0 && h > 0 && w > 0 && H > 0 && W > 0, "bad upsample arguments");
   return launch_upsample_bwd(dy, dx, NC, h, w, H, W, (cudaStream_t)stream);
+}
+
+extern "C" size_t ddn_fc_workspace_bytes(int C, int D) { return fc_shape_ok(C, D) ? sizeof(float) * fc_part_floats(C, D) : 0; }
+
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+// the checks both fc entries share: one feature source, the shape, and 16-byte alignment of what the kernels read as float4 /
+// uint4 (every row of C channels then starts aligned, since C is a multiple of FC_CHUNK)
+static int check_fc_entry(const float* feat, const void* feat_hi, const void* feat_lo, int64_t Mimg, int N, int C, int D) {
+  DDN_CHECK_ARG(!feat != !feat_hi, "fc: exactly one feature source: feat, or the bf16 planes feat_hi (+ feat_lo)");
+  DDN_CHECK_ARG(feat_hi || !feat_lo, "fc: feat_lo is the low plane of feat_hi");
+  DDN_CHECK_ARG(Mimg >= 1 && N >= 1, "fc: need N >= 1 and Mimg >= 1 (got N=%d Mimg=%lld)", N, (long long)Mimg);
+  DDN_CHECK_ARG(fc_shape_ok(C, D), "fc: need 1<=D<=32 and C a multiple of %d (got C=%d D=%d)", FC_CHUNK, C, D);
+  DDN_CHECK_ARG(aligned16(feat) && aligned16(feat_hi) && aligned16(feat_lo), "fc: the feature tensors must be 16-byte aligned");
+  return 0;
+}
+
+extern "C" int ddn_fc_forward(const float* feat, const void* feat_hi, const void* feat_lo, const float* w, const float* bias, float* low,
+                              float* low_nhwc, int64_t Mimg, int N, int C, int D, void* stream) {
+  DDN_CHECK_ARG(w && bias && low, "null tensor");
+  DDN_TRY(check_fc_entry(feat, feat_hi, feat_lo, Mimg, N, C, D));
+  return launch_fc_forward(feat, (const __nv_bfloat16*)feat_hi, (const __nv_bfloat16*)feat_lo, w, bias, low, low_nhwc, Mimg, N, C, D,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int ddn_fc_backward(const float* dlow, const float* feat, const void* feat_hi, const void* feat_lo, const float* w, float* dfeat,
+                               float* dw, float* dbias, int64_t Mimg, int N, int C, int D, void* workspace, size_t workspace_bytes,
+                               void* stream) {
+  DDN_CHECK_ARG(dlow && w && dfeat && dw && dbias && workspace, "null tensor");
+  DDN_TRY(check_fc_entry(feat, feat_hi, feat_lo, Mimg, N, C, D));
+  DDN_CHECK_ARG(aligned16(dfeat), "fc: dfeat must be 16-byte aligned");
+  DDN_CHECK_ARG(((uintptr_t)workspace & 3u) == 0 && workspace_bytes >= ddn_fc_workspace_bytes(C, D), "fc: workspace too small or misaligned");
+  return launch_fc_backward(dlow, feat, (const __nv_bfloat16*)feat_hi, (const __nv_bfloat16*)feat_lo, w, dfeat, dw, dbias, (float*)workspace,
+                            Mimg, N, C, D, (cudaStream_t)stream);
 }

@@ -160,6 +160,48 @@ def upsample_bilinear_backward(dy, h, w):
     return dx
 
 
+def _fc_features(feat, feat_lo):
+    """feat [N, ..., C]: fp32, or the bf16 hi plane (with its lo plane feat_lo, or alone) -> (fp32, hi, lo, N, Mimg, C)"""
+    if not isinstance(feat, torch.Tensor) or not feat.is_cuda or not feat.is_contiguous():
+        raise RuntimeError("feat must be a contiguous CUDA tensor: this path has no CPU fallback")
+    n, c = feat.shape[0], feat.shape[-1]
+    if feat.dtype == torch.bfloat16:
+        if feat_lo is not None and (feat_lo.dtype != torch.bfloat16 or feat_lo.shape != feat.shape or not feat_lo.is_contiguous()):
+            raise RuntimeError("feat_lo must be a contiguous bf16 plane of feat's shape")
+        return None, feat, feat_lo, n, feat.numel() // (n * c), c
+    N.require_cuda_f32(feat, "feat")
+    if feat_lo is not None:
+        raise RuntimeError("feat_lo goes with a bf16 hi plane, not with fp32 features")
+    return feat, None, None, n, feat.numel() // (n * c), c
+
+
+def fc_forward(feat, w, bias, feat_lo=None, low=None, low_nhwc=None):
+    """The scoring 1x1 conv + bias.  feat [N, ..., C] channels-last (fp32, or bf16 planes feat = hi + feat_lo), w [D, C], bias [D].
+    low [N, D, Mimg] is allocated when None; low_nhwc [N, Mimg, D] is written only when given.  -> (low, low_nhwc)"""
+    f32, hi, lo, n, mimg, c = _fc_features(feat, feat_lo)
+    N.require_cuda_f32(w, "w"); N.require_cuda_f32(bias, "bias")
+    d = w.shape[0]
+    if low is None:
+        low = torch.empty(n, d, mimg, dtype=torch.float32, device=feat.device)
+    N.check(N.lib.ddn_fc_forward(N.ptr(f32), N.ptr(hi), N.ptr(lo), N.ptr(w), N.ptr(bias), N.ptr(low), N.ptr(low_nhwc), mimg, n, c, d,
+                                 N.stream_ptr()))
+    return low, low_nhwc
+
+
+def fc_backward(dlow, feat, w, feat_lo=None, dfeat=None, dw=None, dbias=None, workspace=None):
+    """dlow [N, D, Mimg] -> (dfeat [N*Mimg, C], dw [D, C], dbias [D]); outputs and the workspace are allocated when None."""
+    f32, hi, lo, n, mimg, c = _fc_features(feat, feat_lo)
+    N.require_cuda_f32(dlow, "dlow"); N.require_cuda_f32(w, "w")
+    d = w.shape[0]
+    dfeat = torch.empty(n * mimg, c, dtype=torch.float32, device=feat.device) if dfeat is None else dfeat
+    dw = torch.empty_like(w) if dw is None else dw
+    dbias = torch.empty(d, dtype=torch.float32, device=feat.device) if dbias is None else dbias
+    ws = _ws(N.lib.ddn_fc_workspace_bytes(c, d), feat.device) if workspace is None else workspace
+    N.check(N.lib.ddn_fc_backward(N.ptr(dlow), N.ptr(f32), N.ptr(hi), N.ptr(lo), N.ptr(w), N.ptr(dfeat), N.ptr(dw), N.ptr(dbias),
+                                  mimg, n, c, d, N.ptr(ws), ws.numel() * ws.element_size(), N.stream_ptr()))
+    return dfeat, dw, dbias
+
+
 def scale_inplace(t, scale):
     N.require_cuda_f32(t, "t")
     N.check(N.lib.ddn_scale_inplace(N.ptr(t), t.numel(), float(scale), N.stream_ptr()))

@@ -116,6 +116,57 @@ def test_workspace_and_argument_checks():
         N.check(-1)
 
 
+def test_fc_entries_refuse_before_any_launch():
+    """ddn_fc_forward / ddn_fc_backward check every argument before the first launch (fake, never dereferenced pointers:
+    each call below fails one check)."""
+    fake = ctypes.c_void_p(1 << 40)                 # 16-byte aligned
+    assert N.lib.ddn_fc_workspace_bytes(512, 3) == 4 * 512 * (3 * 512 + 3)      # 512 slots for the 512-channel trunk
+    assert N.lib.ddn_fc_workspace_bytes(1024, 32) == 4 * 64 * (32 * 1024 + 32)  # 64 for wider ones
+    assert N.lib.ddn_fc_workspace_bytes(2048, 1) == 4 * 64 * (2048 + 1)
+    for C, D in ((640, 3), (256, 3), (0, 3), (512, 0), (512, 33)):
+        assert N.lib.ddn_fc_workspace_bytes(C, D) == 0
+    ws_bytes = N.lib.ddn_fc_workspace_bytes(512, 3)
+
+    def fwd(feat=fake, hi=None, lo=None, w=fake, low=fake, mimg=77, n=3, C=512, D=3):
+        return N.lib.ddn_fc_forward(feat, hi, lo, w, fake, low, fake, mimg, n, C, D, None)
+
+    def bwd(feat=fake, hi=None, lo=None, w=fake, dfeat=fake, mimg=77, n=3, C=512, D=3, ws=fake, nbytes=ws_bytes):
+        return N.lib.ddn_fc_backward(fake, feat, hi, lo, w, dfeat, fake, fake, mimg, n, C, D, ws, nbytes, None)
+
+    def off(nbytes):
+        return ctypes.c_void_p((1 << 40) + nbytes)
+
+    before = N.launch_count()
+    for call in (fwd, bwd):
+        for C in (640, 256):
+            assert call(C=C) == -1 and b"multiple of 512" in N.lib.ddn_last_error()
+        for D in (0, 33):
+            assert call(D=D) == -1 and b"1<=D<=32" in N.lib.ddn_last_error()
+        assert call(feat=None) == -1 and b"exactly one feature source" in N.lib.ddn_last_error()     # no source
+        assert call(hi=fake) == -1 and b"exactly one feature source" in N.lib.ddn_last_error()       # fp32 and planes
+        assert call(lo=fake) == -1 and b"feat_lo" in N.lib.ddn_last_error()                          # lo without hi
+        assert call(feat=None, lo=fake) == -1                                                        # lo alone
+        assert call(n=0) == -1 and call(mimg=0) == -1
+        assert call(w=None) == -1
+        assert call(feat=off(8)) == -1 and b"16-byte" in N.lib.ddn_last_error()
+        assert call(feat=None, hi=off(8)) == -1 and b"16-byte" in N.lib.ddn_last_error()
+        assert call(feat=None, hi=fake, lo=off(4)) == -1 and b"16-byte" in N.lib.ddn_last_error()
+    assert fwd(low=None) == -1
+    assert bwd(dfeat=off(4)) == -1 and b"dfeat" in N.lib.ddn_last_error()
+    assert bwd(nbytes=ws_bytes - 4) == -1 and b"workspace" in N.lib.ddn_last_error()
+    assert bwd(ws=off(2)) == -1 and b"workspace" in N.lib.ddn_last_error()
+    assert bwd(ws=None) == -1
+    assert N.launch_count() == before
+
+
+def test_batchnorm_workspace_covers_every_supported_width():
+    """the standalone BatchNorm entries take the channel counts the kernels take, the network's 2048 included"""
+    for C in (4, 64, 512, 1024, 2048, 4096):
+        assert N.lib.ddn_batchnorm_workspace_bytes(4800, C) > 0, C
+    for C in (6, 1536, 8192, 0):
+        assert N.lib.ddn_batchnorm_workspace_bytes(4800, C) == 0, C
+
+
 def test_product_refuses_cpu_tensors():
     m = pdc_b200.Resnet34_8s(num_classes=3)
     with pytest.raises(RuntimeError, match="CUDA"):
