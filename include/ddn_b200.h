@@ -360,6 +360,63 @@ int ddn_find_best_match(const float* res_b, int64_t stride_p, int64_t stride_c, 
                         const float* mask_b, int64_t* best_uv_masked, float* best_diff_masked,
                         void* scratch, void* stream);
 
+/* Per-match evaluation statistics == DenseCorrespondenceEvaluation.compute_descriptor_match_statistics
+ * (dense_correspondence/evaluation/evaluation.py:1006-1178) for Q ground-truth matches over N image pairs in one call,
+ * with no host synchronisation.  Query i belongs to pair[i] (int64 [Q], 0 <= pair < N); uv_a [Q,2], uv_b [Q,2] int64 (u, v)
+ * pixels, uv_b already clipped and rounded as clip_pixel_to_image_size_and_round (evaluation.py:603-607) does it.
+ *   res_a, res_b   descriptor images [N,H,W,D] fp32, element (n, v, u, c) at n*s[0] + v*s[1] + u*s[2] + c*s[3] with the
+ *                  strides strides_*_host[4] (elements), e.g. the permuted view forward_single_image_tensor returns; 1 <= D <= 32
+ *   mask_b         [N,H,W] fp32, 1 on the object, 0 elsewhere (the dataset's uint8 mask)
+ *   depth_a/b      [N,H,W] fp32 raw sensor units (millimetres; divided by DEPTH_IM_SCALE = 1000.0 in float64)
+ *   K_inv_host     [9] row-major HOST double: inv(K) as pinhole_projection_image_to_world computes it (numpy.linalg.inv,
+ *                  dense_correspondence/correspondence_tools/correspondence_finder.py:123-144)
+ *   poses_*_host   [N,16] row-major HOST doubles, camera-to-world; copied into `scratch` before this returns
+ * nd(p) = sqrt(sum_c (res_b[p,c] - res_a[uv_a,c])^2) is computed in fp32 exactly as numpy does it on a contiguous float32
+ * array (find_best_match, dense_correspondence/network/dense_correspondence_network.py:488-525): squares rounded, numpy's
+ * pairwise summation order.  The threshold t = nd(uv_b) uses the same arithmetic; the reference computes it with
+ * np.linalg.norm (a BLAS dot, evaluation.py:1070), which may differ from it in the last bits.  The masked distance
+ * nd + (1 - mask_b) * 1e6, its comparison with t and its minimum are float64, as in the reference (evaluation.py:1053-1058).
+ * Outputs, one row per query (column indices DDN_MS_* below):
+ *   out_f32 [Q, DDN_MS_NF32], out_f64 [Q, DDN_MS_NF64], out_i64 [Q, DDN_MS_NI64]
+ * A query whose pair index or pixels lie outside [0,N) x image gets NaN in every float column and -1 in every integer
+ * column, and is counted in *bad_queries (DEVICE int64, overwritten); so is a query whose masked distances are all NaN
+ * (NaN descriptors), which has no masked minimum.  An empty mask_b gives a NaN masked fraction (the
+ * reference divides by an integer 0).  Per-block partial sums are added in a fixed order: a second call is bit-identical.
+ * scratch: ddn_match_statistics_scratch_bytes(N, H, W, Q) bytes (0 for sizes outside the limits below). */
+#define DDN_MS_MAX_PAIRS 65535
+#define DDN_MS_MAX_QUERIES (1 << 22)
+enum { DDN_MS_NORM_DIFF_DESCRIPTOR_GROUND_TRUTH = 0, DDN_MS_NORM_DIFF_DESCRIPTOR = 1, DDN_MS_NF32 = 2 };
+enum {
+  DDN_MS_NORM_DIFF_DESCRIPTOR_MASKED = 0,
+  DDN_MS_NORM_DIFF_GROUND_TRUTH_3D = 1,
+  DDN_MS_NORM_DIFF_PRED_3D = 2,
+  DDN_MS_NORM_DIFF_PRED_3D_MASKED = 3,
+  DDN_MS_PIXEL_MATCH_ERROR_L2 = 4,
+  DDN_MS_PIXEL_MATCH_ERROR_L2_MASKED = 5,
+  DDN_MS_PIXEL_MATCH_ERROR_L1 = 6,
+  DDN_MS_FRACTION_CLOSER = 7,                 /* fraction_pixels_closer_than_ground_truth            */
+  DDN_MS_FRACTION_CLOSER_MASKED = 8,          /* fraction_pixels_closer_than_ground_truth_masked     */
+  DDN_MS_AVERAGE_L2_FALSE_POSITIVES = 9,      /* average_l2_distance_for_false_positives             */
+  DDN_MS_AVERAGE_L2_FALSE_POSITIVES_MASKED = 10,
+  DDN_MS_NF64 = 11
+};
+enum {
+  DDN_MS_IS_VALID = 0,
+  DDN_MS_IS_VALID_MASKED = 1,
+  DDN_MS_U_PRED = 2, DDN_MS_V_PRED = 3,                 /* best match (first minimum of nd)              */
+  DDN_MS_U_PRED_MASKED = 4, DDN_MS_V_PRED_MASKED = 5,   /* masked best match                             */
+  DDN_MS_NUM_CLOSER = 6, DDN_MS_NUM_CLOSER_MASKED = 7,  /* pixels with nd < t, with masked nd < t        */
+  DDN_MS_NUM_MASK_PIXELS = 8,                           /* nonzero pixels of mask_b                      */
+  DDN_MS_NI64 = 9
+};
+size_t ddn_match_statistics_scratch_bytes(int N, int H, int W, int64_t Q);
+int ddn_match_statistics(const float* res_a, const int64_t* strides_a_host, const float* res_b, const int64_t* strides_b_host,
+                         int N, int H, int W, int D, const int64_t* pair, const int64_t* uv_a, const int64_t* uv_b, int64_t Q,
+                         const float* mask_b, const float* depth_a, const float* depth_b,
+                         const double* K_inv_host, const double* poses_a_host, const double* poses_b_host,
+                         float* out_f32, double* out_f64, int64_t* out_i64, int64_t* bad_queries,
+                         void* scratch, size_t scratch_bytes, void* stream);
+
 /* Non-match sampling on the device: out_b[j] = flat index (u + W*v) of a pixel drawn uniformly from the nonzero pixels of
  * `mask` [H*W] fp32 (nz[floor(rand_u[j] * #nonzero)], nonzero pixels in ascending order) or, when mask is NULL or empty,
  * from the whole image (floor(rand_u*W), floor(rand_v*H)); out_a[j] = matches_a[j / non_matches_per_match] (may be NULL).

@@ -13,7 +13,9 @@ from .pixelwise_contrastive_loss import PixelwiseContrastiveLoss, DEFAULT_LOSS_C
 from . import loss_composer
 from .loss_composer import SpartanDatasetDataType
 from .fused_adam import FusedAdam, adjust_learning_rate
-from . import ops, synthetic, data_parallel, sampling
+from . import ops, synthetic, data_parallel, sampling, evaluation
+from .evaluation import DenseCorrespondenceEvaluation, match_statistics, quantitative_analysis_on_pair
 
 __all__ = ["Resnet34_8s", "Resnet50_8s", "DenseCorrespondenceNetwork", "PixelwiseContrastiveLoss", "loss_composer",
-           "SpartanDatasetDataType", "DEFAULT_LOSS_CONFIG", "set_default_precision", "FusedAdam", "adjust_learning_rate", "ops", "synthetic", "data_parallel", "sampling"]
+           "SpartanDatasetDataType", "DEFAULT_LOSS_CONFIG", "set_default_precision", "FusedAdam", "adjust_learning_rate", "ops", "synthetic", "data_parallel", "sampling",
+           "evaluation", "DenseCorrespondenceEvaluation", "match_statistics", "quantitative_analysis_on_pair"]

@@ -98,6 +98,9 @@ _SIGNATURES = {
     "ddn_find_pixel_correspondences_scratch_bytes": (sz, [i64]),
     "ddn_find_pixel_correspondences": (i32, [vp, vp, i32, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
     "ddn_find_best_match": (i32, [vp, i64, i64, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ddn_match_statistics_scratch_bytes": (sz, [i32, i32, i32, i64]),
+    "ddn_match_statistics": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                   vp, sz, vp]),
     "ddn_adam_step": (i32, [vp, vp, vp, vp, i64, i64, f32, f32, f32, f32, f32, f32, vp]),
     "ddn_profile_enable": (i32, [i32]),
     "ddn_profile_reset": (i32, []),
