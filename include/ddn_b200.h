@@ -441,6 +441,50 @@ int ddn_find_pixel_correspondences(const float* depth_a, const float* depth_b, i
                                    int64_t* out_a, int64_t* out_b, float* out_u2, float* out_v2, int64_t* out_count,
                                    void* scratch, size_t scratch_bytes, void* stream);
 
+/* Within-scene training batch on the device == SpartanDataset.get_within_scene_data
+ * (dense_correspondence/dataset/spartan_dataset_masked.py:646-769, SINGLE_OBJECT_WITHIN_SCENE, debug off) for B image pairs
+ * at once, with every random number given as an input.  Per pair: candidates in A (from mask_a when
+ * sample_matches_only_off_mask, else uniform), reprojection into B (as ddn_find_pixel_correspondences), background domain
+ * randomisation of A then B (correspondence_augmentation.py:86-214, exact uint8 arithmetic), the 180-degree flip of A and B
+ * with their index lists, masked / background non-matches from the flipped mask_b, blind non-matches, and
+ * ToTensor + Normalize into fp32 NCHW.  A pair whose mask_a is empty while sampling on the mask is the reference's
+ * return_empty_data: both images are the normalised, un-augmented image A and every count is 0.
+ * Index outputs are [B, cap] int64 padded with -1 past the pair's count: cap = n_attempts (matches),
+ * n_attempts * k_masked, n_attempts * k_background, H * W (blind).  counts [B, 4] int64 (matches, masked, background, blind)
+ * and empty [B] uint8 are DEVICE outputs: nothing is read back, and the number of launches does not depend on B.
+ * Every device array is dense in the layout given below; K [9], poses [B * 16] are row-major HOST doubles. */
+#define DDN_WS_MAX_PAIRS 128          /* per-pair matrices travel as kernel parameters (168 bytes each) */
+enum { DDN_WS_RANDOMIZE = 0, DDN_WS_GRADIENT, DDN_WS_VERTICAL, DDN_WS_NOISE, DDN_WS_FLIP, DDN_WS_RGB1, DDN_WS_RGB2 = 8,
+       DDN_WS_PARAM_BYTES = 16 };    /* byte offsets in one image's parameter block */
+typedef struct {
+  int32_t B, H, W;
+  int32_t sample_matches_only_off_mask, domain_randomize, use_image_b_mask_inv;
+  int64_t n_attempts, k_masked, k_background;
+  float mean[3], std[3];              /* Normalize, per channel */
+} ddn_ws_batch_cfg;
+typedef struct {
+  /* [B, 2, DDN_WS_PARAM_BYTES] uint8, image A then B: decisions (0 / 1) at DDN_WS_RANDOMIZE..DDN_WS_FLIP, colours
+   * rgb1 / rgb2 (0..254) at DDN_WS_RGB1 / DDN_WS_RGB2; the solid background uses rgb1 */
+  const uint8_t* params;
+  const uint8_t* noise;               /* [B, 2 (image), 2 (N1, N2), H, W, 3] uint8: background + N1 - N2 */
+  const float *cand_u, *cand_v;       /* [B, n_attempts] uniform [0, 1) */
+  const float *masked_u, *masked_v;   /* [B, n_attempts * k_masked] */
+  const float *background_u, *background_v;  /* [B, n_attempts * k_background] */
+  const float* blind;                 /* [B, H * W] */
+} ddn_ws_batch_rand;
+typedef struct {
+  float *image_a, *image_b;           /* [B, 3, H, W] */
+  int64_t *matches_a, *matches_b, *masked_a, *masked_b, *background_a, *background_b, *blind_a, *blind_b;
+  int64_t* counts;                    /* [B, 4] */
+  uint8_t* empty;                     /* [B] */
+} ddn_ws_batch_out;
+size_t ddn_within_scene_batch_scratch_bytes(const ddn_ws_batch_cfg* cfg);   /* 0 for a refused cfg */
+int ddn_within_scene_batch(const ddn_ws_batch_cfg* cfg, const uint8_t* rgb_a, const uint8_t* rgb_b,
+                           const uint8_t* mask_a, const uint8_t* mask_b, const float* depth_a, const float* depth_b,
+                           const double* K_host, const double* poses_a_host, const double* poses_b_host,
+                           const ddn_ws_batch_rand* rand, const ddn_ws_batch_out* out,
+                           void* scratch, size_t scratch_bytes, void* stream);
+
 /* Fused Adam step over flat arrays == torch.optim.Adam(lr, betas, eps, weight_decay) as used by
  * dense_correspondence/training/training.py:133-145,346 (L2 weight decay folded into the gradient, bias-corrected moments,
  * no amsgrad).  `step` is the 1-based step count; grads are read as grads[i]*grad_scale (1/world after a SUM all-reduce). */

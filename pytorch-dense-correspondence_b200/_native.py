@@ -44,6 +44,26 @@ class WithinSceneCfg(ctypes.Structure):
                 ("len_match", vp), ("len_masked", vp), ("len_background", vp), ("len_blind", vp)]
 
 
+class WsBatchCfg(ctypes.Structure):
+    _fields_ = [("B", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32),
+                ("sample_matches_only_off_mask", ctypes.c_int32), ("domain_randomize", ctypes.c_int32),
+                ("use_image_b_mask_inv", ctypes.c_int32), ("n_attempts", i64), ("k_masked", i64), ("k_background", i64),
+                ("mean", f32 * 3), ("std", f32 * 3)]
+
+
+class WsBatchRand(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("params", "noise", "cand_u", "cand_v", "masked_u", "masked_v", "background_u",
+                                  "background_v", "blind")]
+
+
+class WsBatchOut(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("image_a", "image_b", "matches_a", "matches_b", "masked_a", "masked_b", "background_a",
+                                  "background_b", "blind_a", "blind_b", "counts", "empty")]
+
+
+WS_MAX_PAIRS = 128
+WS_RANDOMIZE, WS_GRADIENT, WS_VERTICAL, WS_NOISE, WS_FLIP, WS_RGB1, WS_RGB2, WS_PARAM_BYTES = 0, 1, 2, 3, 4, 5, 8, 16
+
 _SIGNATURES = {
     "ddn_abi_version": (i32, []),
     "ddn_set_reserved_sms": (i32, [i32]),
@@ -97,6 +117,9 @@ _SIGNATURES = {
     "ddn_sample_non_matches": (i32, [vp, i32, i32, vp, vp, i64, vp, i64, vp, vp, vp, sz, vp]),
     "ddn_find_pixel_correspondences_scratch_bytes": (sz, [i64]),
     "ddn_find_pixel_correspondences": (i32, [vp, vp, i32, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
+    "ddn_within_scene_batch_scratch_bytes": (sz, [ctypes.POINTER(WsBatchCfg)]),
+    "ddn_within_scene_batch": (i32, [ctypes.POINTER(WsBatchCfg)] + [vp] * 9 + [ctypes.POINTER(WsBatchRand),
+                                     ctypes.POINTER(WsBatchOut), vp, sz, vp]),
     "ddn_find_best_match": (i32, [vp, i64, i64, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ddn_match_statistics_scratch_bytes": (sz, [i32, i32, i32, i64]),
     "ddn_match_statistics": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,

@@ -8,114 +8,8 @@
 // at correspondence_finder.py:354 makes need_to_be_perturbed identically zero); it is reproduced as that no-op.
 // The uniform random numbers are an INPUT (torch.rand on the device), which makes the op bit-reproducible against the
 // restated reference given the same numbers.
-#include "common.cuh"
-
-namespace ddn {
-
-constexpr int SAMP_THREADS = 256;
-constexpr int SAMP_PER_BLOCK = 1024;     // pixels per block in the compaction passes
-
-__global__ void __launch_bounds__(SAMP_THREADS)
-mask_count_kernel(const float* __restrict__ mask, int64_t P, int* __restrict__ block_counts) {
-  pdl_prologue();
-  const int64_t base = (int64_t)blockIdx.x * SAMP_PER_BLOCK;
-  int c = 0;
-#pragma unroll
-  for (int i = 0; i < SAMP_PER_BLOCK / SAMP_THREADS; ++i) {
-    int64_t p = base + i * SAMP_THREADS + threadIdx.x;
-    c += (p < P && mask[p] != 0.f) ? 1 : 0;
-  }
-  c = warp_sum(c);
-  __shared__ int s[SAMP_THREADS / 32];
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int t = 0;
-    for (int i = 0; i < SAMP_THREADS / 32; ++i) t += s[i];
-    block_counts[blockIdx.x] = t;
-  }
-}
-
-// exclusive scan of up to 8192 block counts by one block; total -> counts[nblk]
-__global__ void __launch_bounds__(1024)
-mask_scan_kernel(int* __restrict__ counts, int nblk) {
-  pdl_prologue();
-  __shared__ int s[1024];
-  __shared__ int carry;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int base = 0; base < nblk; base += 1024) {
-    int i = base + threadIdx.x;
-    int v = i < nblk ? counts[i] : 0;
-    s[threadIdx.x] = v;
-    __syncthreads();
-    for (int off = 1; off < 1024; off <<= 1) {
-      int t = threadIdx.x >= off ? s[threadIdx.x - off] : 0;
-      __syncthreads();
-      s[threadIdx.x] += t;
-      __syncthreads();
-    }
-    int incl = s[threadIdx.x];
-    if (i < nblk) counts[i] = carry + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry += incl;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) counts[nblk] = carry;
-}
-
-// ascending list of the nonzero pixels (== torch.nonzero order)
-__global__ void __launch_bounds__(SAMP_THREADS)
-mask_compact_kernel(const float* __restrict__ mask, int64_t P, const int* __restrict__ block_offsets, int* __restrict__ nz) {
-  pdl_prologue();
-  const int64_t base = (int64_t)blockIdx.x * SAMP_PER_BLOCK;
-  __shared__ int warp_tot[SAMP_PER_BLOCK / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  bool f[SAMP_PER_BLOCK / SAMP_THREADS];
-  int rank[SAMP_PER_BLOCK / SAMP_THREADS];
-#pragma unroll
-  for (int i = 0; i < SAMP_PER_BLOCK / SAMP_THREADS; ++i) {
-    int64_t p = base + i * SAMP_THREADS + threadIdx.x;
-    f[i] = p < P && mask[p] != 0.f;
-    unsigned b = __ballot_sync(0xffffffffu, f[i]);
-    rank[i] = __popc(b & ((1u << lane) - 1u));
-    if (lane == 0) warp_tot[i * (SAMP_THREADS / 32) + wid] = __popc(b);
-  }
-  __syncthreads();
-  // segment order inside the block: (i, wid) ascending == pixel order
-#pragma unroll
-  for (int i = 0; i < SAMP_PER_BLOCK / SAMP_THREADS; ++i) {
-    if (!f[i]) continue;
-    int seg = i * (SAMP_THREADS / 32) + wid, before = 0;
-    for (int k = 0; k < seg; ++k) before += warp_tot[k];
-    nz[block_offsets[blockIdx.x] + before + rank[i]] = (int)(base + i * SAMP_THREADS + threadIdx.x);
-  }
-}
-
-__global__ void __launch_bounds__(SAMP_THREADS)
-sample_non_matches_kernel(const int* __restrict__ nz, const int* __restrict__ total, const float* __restrict__ rand_u,
-                          const float* __restrict__ rand_v, int64_t n, int H, int W, const int64_t* __restrict__ matches_a,
-                          int64_t k, int64_t* __restrict__ out_a, int64_t* __restrict__ out_b) {
-  pdl_prologue();
-  const int L = total ? total[0] : 0;
-  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
-    int64_t b;
-    if (L > 0) {
-      int r = (int)floorf(rand_u[j] * (float)L);      // torch.rand(n) * len(mask_b_indices_flat) -> floor -> long
-      if (r >= L) r = L - 1;                          // fp32 rounding at rand ~ 1: the reference's index_select would raise here
-      b = nz[r];
-    } else {                                           // no / empty mask: pytorch_rand_select_pixel (finder.py:64-75)
-      int u = (int)floorf(rand_u[j] * (float)W), v = (int)floorf(rand_v[j] * (float)H);
-      if (u >= W) u = W - 1;
-      if (v >= H) v = H - 1;
-      b = (int64_t)u + (int64_t)W * v;
-    }
-    out_b[j] = b;
-    if (out_a) out_a[j] = matches_a[j / k];
-  }
-}
-
-}  // namespace ddn
+// The kernels (sampling.cuh) work on rows of image pairs; the two entry points here are a batch of one.
+#include "sampling.cuh"
 
 using namespace ddn;
 
@@ -132,92 +26,44 @@ extern "C" int ddn_sample_non_matches(const float* mask, int H, int W, const flo
   if (n == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t P = (int64_t)H * W;
-  int* nz = nullptr; int* total = nullptr;
+  SampleRows s = {};
   if (mask) {
     DDN_CHECK_ARG(scratch && scratch_bytes >= ddn_sample_non_matches_scratch_bytes(H, W), "scratch too small");
     const int nblk = (int)ceil_div(P, SAMP_PER_BLOCK);
     DDN_CHECK_ARG(nblk <= 1 << 20, "image too large");
     int* counts = reinterpret_cast<int*>(scratch);      // [nblk + 1]
-    nz = counts + nblk + 8;
-    DDN_LAUNCH(mask_count_kernel, nblk, SAMP_THREADS, 0, st, mask, P, counts);
-    DDN_LAUNCH(mask_scan_kernel, 1, 1024, 0, st, counts, nblk);
-    DDN_LAUNCH(mask_compact_kernel, nblk, SAMP_THREADS, 0, st, mask, P, counts, nz);
-    total = counts + nblk;
+    const CompactRows c = {counts, counts + nblk + 8, 0, 0, nblk};
+    DDN_TRY(compact_rows(NonzeroF32{mask, P}, P, 1, c, st));
+    s.nz = c.nz; s.counts = counts; s.nblk = nblk;
   }
+  s.ru = rand_u; s.rv = rand_v; s.n = n; s.k = out_a ? non_matches_per_match : 1;
+  s.matches_a = matches_a; s.out_a = out_a; s.out_b = out_b; s.H = H; s.W = W;
   int blocks = (int)std::min<int64_t>(ceil_div(n, SAMP_THREADS), (int64_t)num_sms() * 8);
-  DDN_LAUNCH(sample_non_matches_kernel, blocks, SAMP_THREADS, 0, st, nz, total, rand_u, rand_v, n, H, W, matches_a,
-             non_matches_per_match, out_a, out_b);
+  DDN_LAUNCH(sample_non_matches_kernel, blocks, SAMP_THREADS, 0, st, s);
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
-// Pinhole reprojection match finder (SURVEY.md 8f row 3) == batch_find_pixel_correspondences
-// (dense_correspondence/correspondence_tools/correspondence_finder.py:409-619) for candidate pixels already drawn in image A:
-// depth lookup (uint16 millimetres / DEPTH_IM_SCALE=1000, constants.py:10) -> K^-1 -> pose_a -> pose_b^-1 -> K -> (u2, v2),
-// prune zero depth, out-of-frustum (including the reference's quirk that an exact 0.0 coordinate is pruned by nonzero()),
-// and occlusion against depth image B with the 3 mm margin; survivors keep their order (stream compaction).
+// Pinhole reprojection match finder: see sampling.cuh.
 namespace ddn {
 
-struct ReprojMats { float Kinv[9]; float Ta[12]; float Tb_inv[12]; float K[9]; };
-
-__device__ __forceinline__ void mat3_apply(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-  ox = M[0] * x + M[1] * y + M[2] * z;
-  oy = M[3] * x + M[4] * y + M[5] * z;
-  oz = M[6] * x + M[7] * y + M[8] * z;
-}
-__device__ __forceinline__ void rigid_apply(const float* T, float x, float y, float z, float& ox, float& oy, float& oz) {
-  ox = T[0] * x + T[1] * y + T[2] * z + T[3];
-  oy = T[4] * x + T[5] * y + T[6] * z + T[7];
-  oz = T[8] * x + T[9] * y + T[10] * z + T[11];
-}
-
-__global__ void __launch_bounds__(SAMP_THREADS)
-reproject_kernel(const float* __restrict__ depth_a, const float* __restrict__ depth_b, const int64_t* __restrict__ cand, int64_t n,
-                 int H, int W, const __grid_constant__ ReprojMats m, float* __restrict__ flag, int64_t* __restrict__ b_flat,
-                 float* __restrict__ u2o, float* __restrict__ v2o) {
-  pdl_prologue();
-  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t ia = cand[j];
-    float ok = 0.f; int64_t bf = 0; float u2 = 0.f, v2 = 0.f;
-    if (ia >= 0 && ia < (int64_t)H * W) {
-      const float depth = depth_a[ia] * 1.0f / 1000.0f;
-      if (depth != 0.f) {
-        const float u = (float)(ia % W), v = (float)(ia / W);
-        float cx, cy, cz, wx, wy, wz, px, py, pz, qx, qy, qz;
-        mat3_apply(m.Kinv, u * depth, v * depth, depth, cx, cy, cz);
-        rigid_apply(m.Ta, cx, cy, cz, wx, wy, wz);
-        rigid_apply(m.Tb_inv, wx, wy, wz, px, py, pz);
-        mat3_apply(m.K, px, py, pz, qx, qy, qz);
-        u2 = qx / qz; v2 = qy / qz;
-        const float z2 = qz;
-        const float ub = (float)W * 1.0f - 1e-3f, vb = (float)H * 1.0f - 1e-3f;
-        bool in = !(u2 < 0.f) && !(u2 > ub) && u2 != 0.f && !(v2 < 0.f) && !(v2 > vb) && v2 != 0.f;
-        if (in && u2 == u2 && v2 == v2) {
-          bf = (int64_t)v2 * W + (int64_t)u2;                 // .type(long): truncation
-          float d2 = depth_b[bf] * 1.0f / 1000.0f;
-          if (d2 < 0.f) d2 = 0.f;
-          if (d2 < z2 - 0.003f) d2 = 0.f;                      // occluded in image b
-          ok = d2 != 0.f ? 1.f : 0.f;
-        }
-      }
-    }
-    flag[j] = ok; b_flat[j] = bf; u2o[j] = u2; v2o[j] = v2;
+bool reproj_mats(const double* K, const double* pose_a, const double* pose_b, ReprojMats& m) {
+  const double det = K[0] * (K[4] * K[8] - K[5] * K[7]) - K[1] * (K[3] * K[8] - K[5] * K[6]) + K[2] * (K[3] * K[7] - K[4] * K[6]);
+  if (det == 0.0) return false;
+  const double inv[9] = {(K[4] * K[8] - K[5] * K[7]) / det, (K[2] * K[7] - K[1] * K[8]) / det, (K[1] * K[5] - K[2] * K[4]) / det,
+                         (K[5] * K[6] - K[3] * K[8]) / det, (K[0] * K[8] - K[2] * K[6]) / det, (K[2] * K[3] - K[0] * K[5]) / det,
+                         (K[3] * K[7] - K[4] * K[6]) / det, (K[1] * K[6] - K[0] * K[7]) / det, (K[0] * K[4] - K[1] * K[3]) / det};
+  for (int i = 0; i < 9; ++i) { m.Kinv[i] = (float)inv[i]; m.K[i] = (float)K[i]; }
+  for (int i = 0; i < 12; ++i) m.Ta[i] = (float)pose_a[i];
+  // invert_transform (correspondence_finder.py:52-62): [R^T | -R^T t] in double, then cast to fp32
+  const double* P = pose_b;
+  const double Rt[9] = {P[0], P[4], P[8], P[1], P[5], P[9], P[2], P[6], P[10]};
+  const double t[3] = {P[3], P[7], P[11]};
+  for (int r = 0; r < 3; ++r) {
+    m.Tb_inv[r * 4 + 0] = (float)Rt[r * 3 + 0]; m.Tb_inv[r * 4 + 1] = (float)Rt[r * 3 + 1]; m.Tb_inv[r * 4 + 2] = (float)Rt[r * 3 + 2];
+    m.Tb_inv[r * 4 + 3] = (float)(-1.0 * (Rt[r * 3 + 0] * t[0] + Rt[r * 3 + 1] * t[1] + Rt[r * 3 + 2] * t[2]));
   }
-}
-
-__global__ void __launch_bounds__(SAMP_THREADS)
-reproject_gather_kernel(const int* __restrict__ nz, const int* __restrict__ total, const int64_t* __restrict__ cand,
-                        const int64_t* __restrict__ b_flat, const float* __restrict__ u2, const float* __restrict__ v2,
-                        int64_t* __restrict__ out_a, int64_t* __restrict__ out_b, float* __restrict__ out_u2, float* __restrict__ out_v2,
-                        int64_t* __restrict__ out_count) {
-  pdl_prologue();
-  const int L = total[0];
-  if (blockIdx.x == 0 && threadIdx.x == 0) out_count[0] = L;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < L; i += gridDim.x * blockDim.x) {
-    const int j = nz[i];
-    out_a[i] = cand[j]; out_b[i] = b_flat[j];
-    if (out_u2) { out_u2[i] = u2[j]; out_v2[i] = v2[j]; }
-  }
+  return true;
 }
 
 }  // namespace ddn
@@ -239,39 +85,24 @@ extern "C" int ddn_find_pixel_correspondences(const float* depth_a, const float*
   DDN_CHECK_ARG(H > 0 && W > 0 && n > 0 && n < (1ll << 30) && scratch_bytes >= ddn_find_pixel_correspondences_scratch_bytes(n),
                 "bad sizes / scratch too small");
   cudaStream_t st = (cudaStream_t)stream;
-  // host-side matrix prep in double, exactly like the reference's numpy (inv(K), invert_transform(pose_b)), then cast to fp32
-  ReprojMats m;
-  const double* K = K_host;
-  const double det = K[0] * (K[4] * K[8] - K[5] * K[7]) - K[1] * (K[3] * K[8] - K[5] * K[6]) + K[2] * (K[3] * K[7] - K[4] * K[6]);
-  DDN_CHECK_ARG(det != 0.0, "singular intrinsics");
-  const double inv[9] = {(K[4] * K[8] - K[5] * K[7]) / det, (K[2] * K[7] - K[1] * K[8]) / det, (K[1] * K[5] - K[2] * K[4]) / det,
-                         (K[5] * K[6] - K[3] * K[8]) / det, (K[0] * K[8] - K[2] * K[6]) / det, (K[2] * K[3] - K[0] * K[5]) / det,
-                         (K[3] * K[7] - K[4] * K[6]) / det, (K[1] * K[6] - K[0] * K[7]) / det, (K[0] * K[4] - K[1] * K[3]) / det};
-  for (int i = 0; i < 9; ++i) { m.Kinv[i] = (float)inv[i]; m.K[i] = (float)K[i]; }
-  for (int i = 0; i < 12; ++i) m.Ta[i] = (float)pose_a_host[i];
-  // invert_transform (correspondence_finder.py:52-62): [R^T | -R^T t] in double, then cast to fp32
-  {
-    const double* P = pose_b_host;
-    const double Rt[9] = {P[0], P[4], P[8], P[1], P[5], P[9], P[2], P[6], P[10]};
-    const double t[3] = {P[3], P[7], P[11]};
-    for (int r = 0; r < 3; ++r) {
-      m.Tb_inv[r * 4 + 0] = (float)Rt[r * 3 + 0]; m.Tb_inv[r * 4 + 1] = (float)Rt[r * 3 + 1]; m.Tb_inv[r * 4 + 2] = (float)Rt[r * 3 + 2];
-      m.Tb_inv[r * 4 + 3] = (float)(-1.0 * (Rt[r * 3 + 0] * t[0] + Rt[r * 3 + 1] * t[1] + Rt[r * 3 + 2] * t[2]));
-    }
-  }
+  ReprojBatch<1> mats;
+  DDN_CHECK_ARG(reproj_mats(K_host, pose_a_host, pose_b_host, mats.m[0]), "singular intrinsics");
   char* p = reinterpret_cast<char*>(align_up(reinterpret_cast<uintptr_t>(scratch), 16));
   float* flag = (float*)p; p += align_up((size_t)n * 4, 16);
   int64_t* b_flat = (int64_t*)p; p += align_up((size_t)n * 8, 16);
   float* u2 = (float*)p; p += align_up((size_t)n * 4, 16);
   float* v2 = (float*)p; p += align_up((size_t)n * 4, 16);
   const int nblk = (int)ceil_div(n, SAMP_PER_BLOCK);
-  int* counts = (int*)p; int* nz = counts + nblk + 8;
+  int* counts = (int*)p;
+  const CompactRows c = {counts, counts + nblk + 8, 0, 0, nblk};
   int blocks = (int)std::min<int64_t>(ceil_div(n, SAMP_THREADS), (int64_t)num_sms() * 8);
-  DDN_LAUNCH(reproject_kernel, blocks, SAMP_THREADS, 0, st, depth_a, depth_b, candidates, n, H, W, m, flag, b_flat, u2, v2);
-  DDN_LAUNCH(mask_count_kernel, nblk, SAMP_THREADS, 0, st, flag, n, counts);
-  DDN_LAUNCH(mask_scan_kernel, 1, 1024, 0, st, counts, nblk);
-  DDN_LAUNCH(mask_compact_kernel, nblk, SAMP_THREADS, 0, st, flag, n, counts, nz);
-  DDN_LAUNCH(reproject_gather_kernel, blocks, SAMP_THREADS, 0, st, nz, counts + nblk, candidates, b_flat, u2, v2, out_a, out_b, out_u2,
-             out_v2, out_count);
+  DDN_LAUNCH(reproject_kernel<1>, blocks, SAMP_THREADS, 0, st, depth_a, depth_b, candidates, n, H, W, mats, flag, b_flat, u2, v2);
+  DDN_TRY(compact_rows(NonzeroF32{flag, n}, n, 1, c, st));
+  GatherRows g = {};
+  g.nz = c.nz; g.counts = counts; g.nblk = nblk;
+  g.cand = candidates; g.b_flat = b_flat; g.u2 = u2; g.v2 = v2;
+  g.out_a = out_a; g.out_b = out_b; g.out_u2 = out_u2; g.out_v2 = out_v2; g.out_count = out_count;
+  g.H = H; g.W = W;
+  DDN_LAUNCH(reproject_gather_kernel, blocks, SAMP_THREADS, 0, st, g);
   return 0;
 }

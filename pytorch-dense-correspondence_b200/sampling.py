@@ -61,3 +61,127 @@ def find_pixel_correspondences(depth_a, pose_a, depth_b, pose_b, candidates_a, K
                                                  N.ptr(count), N.ptr(scratch), nb, N.stream_ptr()))
     m = int(count.item())
     return out_a[:m], out_b[:m], u2[:m], v2[:m]
+
+
+# ----------------------------------------------------------------------------- within-scene training batches
+# DEFAULT_IMAGE_MEAN / DEFAULT_IMAGE_STD_DEV (modules/dense_correspondence_manipulation/utils/constants.py:18-19): the
+# Normalize of SpartanDataset.rgb_image_to_tensor
+IMAGE_MEAN = (0.5573105812072754, 0.37420374155044556, 0.37020164728164673)
+IMAGE_STD = (0.24336038529872894, 0.2987397611141205, 0.31875079870224)
+
+_RAND_KEYS = ("cand_u", "cand_v", "masked_u", "masked_v", "background_u", "background_v", "blind")
+
+
+def within_scene_cfg(training_config):
+    """The ``training`` section of a training config -> the sampling sizes of SpartanDataset
+    (dense_correspondence_dataset_masked.py:538-551): k = int(fraction * num_non_matches_per_match)."""
+    t = training_config["training"]
+    nn = t["num_non_matches_per_match"]
+    return dict(n_attempts=int(t["num_matching_attempts"]), k_masked=int(t["fraction_masked_non_matches"] * nn),
+                k_background=int(t["fraction_background_non_matches"] * nn),
+                sample_matches_only_off_mask=bool(t["sample_matches_only_off_mask"]),
+                domain_randomize=bool(t["domain_randomize"]), use_image_b_mask_inv=bool(t["use_image_b_mask_inv"]))
+
+
+def _rand_shapes(B, H, W, c):
+    n = c["n_attempts"]
+    return {"cand_u": (B, n), "cand_v": (B, n), "masked_u": (B, n * c["k_masked"]), "masked_v": (B, n * c["k_masked"]),
+            "background_u": (B, n * c["k_background"]), "background_v": (B, n * c["k_background"]), "blind": (B, H * W)}
+
+
+def draw_within_scene_rand(B, H, W, training_config, generator=None, device=None):
+    """Every random number ``within_scene_batch`` consumes for B pairs of H x W images, drawn on the device.
+    -> dict: ``params`` uint8 [B, 2, 16] (image A, B: randomise / gradient / vertical / noise / flip decisions in {0, 1} at
+    bytes 0-4, colours rgb1 at 5-7 and rgb2 at 8-10 in 0..254, the reference's uint8(U * 255)), ``noise`` uint8
+    [B, 2, 2, H, W, 3] in 0..49 (uint8(U * 50)), and the uniform fp32 arrays ``cand_u/v`` [B, n_attempts],
+    ``masked_u/v`` [B, n_attempts * k_masked], ``background_u/v`` [B, n_attempts * k_background], ``blind`` [B, H * W]."""
+    c = within_scene_cfg(training_config)
+    dev = torch.device(device) if device is not None else (generator.device if generator is not None else torch.device("cuda"))
+    params = torch.zeros(B, 2, N.WS_PARAM_BYTES, dtype=torch.uint8, device=dev)
+    params[:, :, :N.WS_RGB1] = torch.randint(0, 2, (B, 2, N.WS_RGB1), dtype=torch.uint8, device=dev, generator=generator)
+    params[:, :, N.WS_RGB1:N.WS_RGB2 + 3] = torch.randint(0, 255, (B, 2, 6), dtype=torch.uint8, device=dev, generator=generator)
+    out = {"params": params,
+           "noise": torch.randint(0, 50, (B, 2, 2, H, W, 3), dtype=torch.uint8, device=dev, generator=generator)}
+    shapes = _rand_shapes(B, H, W, c)
+    sizes = [shapes[k][0] * shapes[k][1] for k in _RAND_KEYS]
+    flat = torch.rand(sum(sizes), device=dev, generator=generator)
+    for k, part in zip(_RAND_KEYS, torch.split(flat, sizes)):
+        out[k] = part.view(shapes[k])
+    return out
+
+
+def _require(t, name, dtype, shape):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor: this path has no CPU fallback" % name)
+    if t.dtype != dtype:
+        raise RuntimeError("%s must be %s (got %s)" % (name, dtype, t.dtype))
+    if tuple(t.shape) != tuple(shape):
+        raise RuntimeError("%s must have shape %s (got %s)" % (name, tuple(shape), tuple(t.shape)))
+    return t.contiguous()
+
+
+def within_scene_batch(rgb_a, rgb_b, depth_a, depth_b, mask_a, mask_b, pose_a, pose_b, K, training_config, generator=None,
+                       rand=None):
+    """SpartanDataset.get_within_scene_data (dataset/spartan_dataset_masked.py:646-769, SINGLE_OBJECT_WITHIN_SCENE) for B
+    image pairs on the device, in one call that never synchronises with the host.
+
+    rgb_*: uint8 [B, H, W, 3]; mask_*: uint8 [B, H, W] (nonzero = object, any value); depth_*: float32 [B, H, W] in
+    millimetres; all CUDA.  pose_*: [B, 4, 4] camera-to-world (host, numpy or CPU tensor); K: 3x3 intrinsics.
+    ``training_config``: a config with the reference's ``training`` section.  The random numbers are ``rand`` (as returned
+    by ``draw_within_scene_rand``) or are drawn from ``generator``.
+    -> dict: ``image_a`` / ``image_b`` float32 [B, 3, H, W] (augmented, flipped, normalised); ``matches_a/b``,
+    ``masked_non_matches_a/b``, ``background_non_matches_a/b``, ``blind_non_matches_a/b`` int64 [B, cap] padded with -1;
+    ``num_valid`` (the ``get_loss`` argument); ``counts`` int64 [B, 4]; ``empty`` bool [B] (the reference's
+    return_empty_data: mask_a empty while sampling on it); ``match_type`` (CPU, SINGLE_OBJECT_WITHIN_SCENE per pair)."""
+    import ctypes
+    import numpy as np
+    from .loss_composer import SpartanDatasetDataType
+    if training_config.get("training", {}).get("debug", False):
+        raise NotImplementedError("within_scene_batch: debug=True (plotting) is not supported")
+    c = within_scene_cfg(training_config)
+    if not isinstance(rgb_a, torch.Tensor) or rgb_a.dim() != 4:
+        raise RuntimeError("rgb_a must be a uint8 CUDA tensor [B, H, W, 3]")
+    B, H, W = rgb_a.shape[:3]
+    if not 1 <= B <= N.WS_MAX_PAIRS:
+        raise RuntimeError("within_scene_batch takes 1 to %d pairs per call (got %d)" % (N.WS_MAX_PAIRS, B))
+    dev = rgb_a.device
+    rgb_a = _require(rgb_a, "rgb_a", torch.uint8, (B, H, W, 3)); rgb_b = _require(rgb_b, "rgb_b", torch.uint8, (B, H, W, 3))
+    mask_a = _require(mask_a, "mask_a", torch.uint8, (B, H, W)); mask_b = _require(mask_b, "mask_b", torch.uint8, (B, H, W))
+    depth_a = _require(depth_a, "depth_a", torch.float32, (B, H, W)); depth_b = _require(depth_b, "depth_b", torch.float32, (B, H, W))
+    Kd = np.ascontiguousarray(np.asarray(K, dtype=np.float64).reshape(9))
+    Pa = np.ascontiguousarray(np.asarray(pose_a, dtype=np.float64))
+    Pb = np.ascontiguousarray(np.asarray(pose_b, dtype=np.float64))
+    if Pa.shape != (B, 4, 4) or Pb.shape != (B, 4, 4):
+        raise RuntimeError("pose_a / pose_b must have shape [B, 4, 4]")
+    if rand is None:
+        rand = draw_within_scene_rand(B, H, W, training_config, generator=generator, device=dev)
+    shapes = dict(_rand_shapes(B, H, W, c), params=(B, 2, N.WS_PARAM_BYTES), noise=(B, 2, 2, H, W, 3))
+    rand = {k: _require(rand[k], "rand[%r]" % k, torch.uint8 if k in ("params", "noise") else torch.float32, shapes[k])
+            for k in shapes}
+    n, cap_m, cap_b = c["n_attempts"], shapes["masked_u"][1], shapes["background_u"][1]
+    i64 = dict(dtype=torch.int64, device=dev)
+    out = {"image_a": torch.empty(B, 3, H, W, device=dev), "image_b": torch.empty(B, 3, H, W, device=dev),
+           "matches_a": torch.empty(B, n, **i64), "matches_b": torch.empty(B, n, **i64),
+           "masked_non_matches_a": torch.empty(B, cap_m, **i64), "masked_non_matches_b": torch.empty(B, cap_m, **i64),
+           "background_non_matches_a": torch.empty(B, cap_b, **i64), "background_non_matches_b": torch.empty(B, cap_b, **i64),
+           "blind_non_matches_a": torch.empty(B, H * W, **i64), "blind_non_matches_b": torch.empty(B, H * W, **i64),
+           "counts": torch.empty(B, 4, **i64), "empty": torch.empty(B, dtype=torch.bool, device=dev)}
+    cfg = N.WsBatchCfg(B, H, W, int(c["sample_matches_only_off_mask"]), int(c["domain_randomize"]),
+                       int(c["use_image_b_mask_inv"]), n, c["k_masked"], c["k_background"],
+                       (ctypes.c_float * 3)(*IMAGE_MEAN), (ctypes.c_float * 3)(*IMAGE_STD))
+    r = N.WsBatchRand(*[rand[k].data_ptr() or None for k in ("params", "noise") + _RAND_KEYS])
+    o = N.WsBatchOut(*[out[k].data_ptr() or None for k in (
+        "image_a", "image_b", "matches_a", "matches_b", "masked_non_matches_a", "masked_non_matches_b",
+        "background_non_matches_a", "background_non_matches_b", "blind_non_matches_a", "blind_non_matches_b", "counts", "empty")])
+    nb = N.lib.ddn_within_scene_batch_scratch_bytes(ctypes.byref(cfg))
+    if nb == 0:
+        raise RuntimeError("within_scene_batch: configuration refused (%s, B=%d, H=%d, W=%d)" % (c, B, H, W))
+    scratch = torch.empty(nb, dtype=torch.uint8, device=dev)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    N.check(N.lib.ddn_within_scene_batch(ctypes.byref(cfg), N.ptr(rgb_a), N.ptr(rgb_b), N.ptr(mask_a), N.ptr(mask_b),
+                                         N.ptr(depth_a), N.ptr(depth_b), vp(Kd), vp(Pa), vp(Pb), ctypes.byref(r),
+                                         ctypes.byref(o), N.ptr(scratch), nb, N.stream_ptr()))
+    cnt = out["counts"].t().contiguous()
+    out["num_valid"] = {"matches": cnt[0], "masked": cnt[1], "background": cnt[2], "blind": cnt[3]}
+    out["match_type"] = torch.full((B,), SpartanDatasetDataType.SINGLE_OBJECT_WITHIN_SCENE, dtype=torch.int64)
+    return out
