@@ -485,6 +485,81 @@ int ddn_within_scene_batch(const ddn_ws_batch_cfg* cfg, const uint8_t* rgb_a, co
                            const ddn_ws_batch_rand* rand, const ddn_ws_batch_out* out,
                            void* scratch, size_t scratch_bytes, void* stream);
 
+/* Across-scene training batch on the device == SpartanDataset.get_across_scene_data
+ * (dense_correspondence/dataset/spartan_dataset_masked.py:1056-1141, debug off), the producer of DIFFERENT_OBJECT and
+ * SINGLE_OBJECT_ACROSS_SCENE pairs, for B image pairs at once with every random number given as an input.  Per pair:
+ * num_samples blind pixels drawn with replacement from the nonzero pixels of mask_a and of mask_b
+ * (random_sample_from_masked_image_torch, correspondence_finder.py:92-121), background domain randomisation of A then B
+ * (as ddn_within_scene_batch, same parameter blocks and noise layout), the 180-degree flip of A and B with their blind
+ * pixels (p -> P-1-p), and ToTensor + Normalize into fp32 NCHW.  A pair whose mask_a or mask_b is empty is the
+ * reference's return_empty_data: both images are the normalised, un-augmented image A, every count is 0 and the blind
+ * rows are -1.  blind_a / blind_b are [B, num_samples] int64; counts [B, 4] int64 (0, 0, 0, blind) and empty [B] uint8 are
+ * DEVICE outputs: nothing is read back, and a call is 5 launches whatever B.  Every array is a dense device array. */
+#define DDN_AS_MAX_PAIRS 16384        /* 2 * B compaction rows on the grid's y dimension */
+typedef struct {
+  int32_t B, H, W;
+  int32_t domain_randomize;
+  int64_t num_samples;                /* training.cross_scene_num_samples, >= 1 */
+  float mean[3], std[3];              /* Normalize, per channel */
+} ddn_as_batch_cfg;
+typedef struct {
+  const uint8_t* params;              /* [B, 2, DDN_WS_PARAM_BYTES] uint8, as ddn_ws_batch_rand.params */
+  const uint8_t* noise;               /* [B, 2, 2, H, W, 3] uint8, as ddn_ws_batch_rand.noise */
+  const float *blind_a, *blind_b;     /* [B, num_samples] uniform [0, 1): the draws over mask_a, mask_b */
+} ddn_as_batch_rand;
+typedef struct {
+  float *image_a, *image_b;           /* [B, 3, H, W] */
+  int64_t *blind_a, *blind_b;         /* [B, num_samples] */
+  int64_t* counts;                    /* [B, 4] */
+  uint8_t* empty;                     /* [B] */
+} ddn_as_batch_out;
+size_t ddn_across_scene_batch_scratch_bytes(const ddn_as_batch_cfg* cfg);   /* 0 for a refused cfg */
+int ddn_across_scene_batch(const ddn_as_batch_cfg* cfg, const uint8_t* rgb_a, const uint8_t* rgb_b,
+                           const uint8_t* mask_a, const uint8_t* mask_b, const ddn_as_batch_rand* rand,
+                           const ddn_as_batch_out* out, void* scratch, size_t scratch_bytes, void* stream);
+
+/* Synthetic multi-object training batch on the device == SpartanDataset.get_synthetic_multi_object_within_scene_data
+ * (dense_correspondence/dataset/spartan_dataset_masked.py:890-1053, SYNTHETIC_MULTI_OBJECT, debug off) for B pairs at
+ * once, with every random number given as an input.  A pair has two within-scene halves, scene A (images a1, a2) and scene
+ * B (b1, b2); every image input is stacked [B, 2 (scene A, scene B), ...].  Per half: candidates in image 1 (from mask_1 when
+ * sample_matches_only_off_mask, else uniform) and their reprojection into image 2 (as ddn_within_scene_batch, no background
+ * randomisation, no flip); the sub-pixel positions in image 2 are truncated (.long()).  Merge 1 of a1 and b1 and merge 2 of
+ * a2 and b2 (correspondence_augmentation.py:217-347), each with its own foreground decision: fg * m + (1 - m) * bg in uint8
+ * arithmetic modulo 256; the background half keeps the matches whose image-1 (merge 1) / image-2 (merge 2) pixel is off
+ * the foreground's mask.  matches = scene A's survivors then scene B's; masked / background non-matches from merged mask 2
+ * = clip(fg_mask_2 + bg_mask_2, 0, 1) with the uint8 sum wrapping.  There are no blind non-matches.  The reference's four
+ * early returns (mask_a1 empty: a1 twice; mask_b1 empty, or a background half fully occluded by merge 1 or 2: b1 twice)
+ * give the normalised image twice, every count 0 and empty = 1.
+ * Index outputs are [B, cap] int64 padded with -1: cap = 2 * n_attempts (matches), 2 * n_attempts * k_masked,
+ * 2 * n_attempts * k_background, 1 (blind, always -1).  counts [B, 4] (matches, masked, background, 0) and empty [B] are
+ * DEVICE outputs; a call is 15 launches whatever B.  K [9] and poses [B * 2 * 16] (image 1 / image 2 of row 2 * pair + half)
+ * are row-major HOST doubles. */
+#define DDN_SMO_MAX_PAIRS (DDN_WS_MAX_PAIRS / 2)   /* two reprojection matrix sets per pair travel as kernel parameters */
+typedef struct {
+  int32_t B, H, W;
+  int32_t sample_matches_only_off_mask, use_image_b_mask_inv;
+  int64_t n_attempts, k_masked, k_background;
+  float mean[3], std[3];              /* Normalize, per channel */
+} ddn_smo_batch_cfg;
+typedef struct {
+  const uint8_t* merge;               /* [B, 2] uint8: 1 = merge 1 / merge 2 puts scene B in the foreground */
+  const float *cand_u, *cand_v;       /* [B, 2 (half), n_attempts] uniform [0, 1) */
+  const float *masked_u, *masked_v;   /* [B, 2 * n_attempts * k_masked] */
+  const float *background_u, *background_v;  /* [B, 2 * n_attempts * k_background] */
+} ddn_smo_batch_rand;
+typedef struct {
+  float *image_a, *image_b;           /* [B, 3, H, W]: merged image 1, merged image 2 */
+  int64_t *matches_a, *matches_b, *masked_a, *masked_b, *background_a, *background_b, *blind_a, *blind_b;
+  int64_t* counts;                    /* [B, 4] */
+  uint8_t* empty;                     /* [B] */
+} ddn_smo_batch_out;
+size_t ddn_synthetic_multi_object_batch_scratch_bytes(const ddn_smo_batch_cfg* cfg);   /* 0 for a refused cfg */
+int ddn_synthetic_multi_object_batch(const ddn_smo_batch_cfg* cfg, const uint8_t* rgb_1, const uint8_t* rgb_2,
+                                     const uint8_t* mask_1, const uint8_t* mask_2, const float* depth_1, const float* depth_2,
+                                     const double* K_host, const double* poses_1_host, const double* poses_2_host,
+                                     const ddn_smo_batch_rand* rand, const ddn_smo_batch_out* out,
+                                     void* scratch, size_t scratch_bytes, void* stream);
+
 /* Fused Adam step over flat arrays == torch.optim.Adam(lr, betas, eps, weight_decay) as used by
  * dense_correspondence/training/training.py:133-145,346 (L2 weight decay folded into the gradient, bias-corrected moments,
  * no amsgrad).  `step` is the 1-based step count; grads are read as grads[i]*grad_scale (1/world after a SUM all-reduce). */

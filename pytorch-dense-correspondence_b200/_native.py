@@ -64,6 +64,40 @@ class WsBatchOut(ctypes.Structure):
 WS_MAX_PAIRS = 128
 WS_RANDOMIZE, WS_GRADIENT, WS_VERTICAL, WS_NOISE, WS_FLIP, WS_RGB1, WS_RGB2, WS_PARAM_BYTES = 0, 1, 2, 3, 4, 5, 8, 16
 
+
+class AsBatchCfg(ctypes.Structure):
+    _fields_ = [("B", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("domain_randomize", ctypes.c_int32),
+                ("num_samples", i64), ("mean", f32 * 3), ("std", f32 * 3)]
+
+
+class AsBatchRand(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("params", "noise", "blind_a", "blind_b")]
+
+
+class AsBatchOut(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("image_a", "image_b", "blind_a", "blind_b", "counts", "empty")]
+
+
+AS_MAX_PAIRS = 16384
+
+
+class SmoBatchCfg(ctypes.Structure):
+    _fields_ = [("B", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32),
+                ("sample_matches_only_off_mask", ctypes.c_int32), ("use_image_b_mask_inv", ctypes.c_int32),
+                ("n_attempts", i64), ("k_masked", i64), ("k_background", i64), ("mean", f32 * 3), ("std", f32 * 3)]
+
+
+class SmoBatchRand(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("merge", "cand_u", "cand_v", "masked_u", "masked_v", "background_u", "background_v")]
+
+
+class SmoBatchOut(ctypes.Structure):
+    _fields_ = [(k, vp) for k in ("image_a", "image_b", "matches_a", "matches_b", "masked_a", "masked_b", "background_a",
+                                  "background_b", "blind_a", "blind_b", "counts", "empty")]
+
+
+SMO_MAX_PAIRS = WS_MAX_PAIRS // 2
+
 _SIGNATURES = {
     "ddn_abi_version": (i32, []),
     "ddn_set_reserved_sms": (i32, [i32]),
@@ -120,6 +154,12 @@ _SIGNATURES = {
     "ddn_within_scene_batch_scratch_bytes": (sz, [ctypes.POINTER(WsBatchCfg)]),
     "ddn_within_scene_batch": (i32, [ctypes.POINTER(WsBatchCfg)] + [vp] * 9 + [ctypes.POINTER(WsBatchRand),
                                      ctypes.POINTER(WsBatchOut), vp, sz, vp]),
+    "ddn_across_scene_batch_scratch_bytes": (sz, [ctypes.POINTER(AsBatchCfg)]),
+    "ddn_across_scene_batch": (i32, [ctypes.POINTER(AsBatchCfg)] + [vp] * 4 + [ctypes.POINTER(AsBatchRand),
+                                     ctypes.POINTER(AsBatchOut), vp, sz, vp]),
+    "ddn_synthetic_multi_object_batch_scratch_bytes": (sz, [ctypes.POINTER(SmoBatchCfg)]),
+    "ddn_synthetic_multi_object_batch": (i32, [ctypes.POINTER(SmoBatchCfg)] + [vp] * 9 + [ctypes.POINTER(SmoBatchRand),
+                                               ctypes.POINTER(SmoBatchOut), vp, sz, vp]),
     "ddn_find_best_match": (i32, [vp, i64, i64, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ddn_match_statistics_scratch_bytes": (sz, [i32, i32, i32, i64]),
     "ddn_match_statistics": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,

@@ -1,5 +1,5 @@
-// Device sampling kernels shared by the single-pair entry points (sampling.cu) and the within-scene batch producer
-// (within_scene.cu).  Every kernel works on ROWS: blockIdx.y (or the row loop) selects one image pair (or one pair x mask),
+// Device sampling kernels shared by the single-pair entry points (sampling.cu) and the within-scene and across-scene batch
+// producers (within_scene.cu, across_scene.cu).  Every kernel works on ROWS: blockIdx.y (or the row loop) selects one image pair (or one pair x mask),
 // and the single-pair entry points are a batch of one row.
 #pragma once
 #include "common.cuh"
@@ -14,6 +14,18 @@ struct NonzeroF32 {
   const float* x; int64_t P;
   __device__ __forceinline__ bool operator()(int64_t r, int64_t p) const { return x[r * P + p] != 0.f; }
 };
+struct NonzeroU8 {
+  const uint8_t* x; int64_t P;
+  __device__ __forceinline__ bool operator()(int64_t r, int64_t p) const { return x[r * P + p] != 0; }
+};
+
+// random_sample_from_masked_image_torch (correspondence_finder.py:92-121) for one number: the r-th of the L >= 1 selected
+// pixels nz[0..L) at floor(r * L), clamped at L - 1 (fp32 rounding at r ~ 1: the reference's index_select would raise there)
+__device__ __forceinline__ int masked_pick(float r, int L, const int* nz) {
+  int q = (int)floorf(r * (float)L);
+  if (q >= L) q = L - 1;
+  return nz[q];
+}
 
 // Per-row layout of a compaction: block counts (then the row total at index nblk) at counts + r * counts_stride,
 // selected pixels at nz + r * nz_stride.
@@ -153,9 +165,7 @@ sample_non_matches_kernel(const SampleRows s) {
     }
     int64_t b;
     if (L > 0) {
-      int q = (int)floorf(rand_u[j] * (float)L);      // torch.rand(n) * len(mask_b_indices_flat) -> floor -> long
-      if (q >= L) q = L - 1;                          // fp32 rounding at rand ~ 1: the reference's index_select would raise here
-      b = nz[q];
+      b = masked_pick(rand_u[j], L, nz);              // torch.rand(n) * len(mask_b_indices_flat) -> floor -> long
     } else {                                           // no / empty mask: pytorch_rand_select_pixel (finder.py:64-75)
       int u = (int)floorf(rand_u[j] * (float)W), v = (int)floorf(rand_v[j] * (float)H);
       if (u >= W) u = W - 1;
@@ -275,6 +285,73 @@ reproject_gather_kernel(const GatherRows g) {
     out_a[i] = a; out_b[i] = b;
     if (g.out_u2) { g.out_u2[r * g.out_stride + i] = u; g.out_v2[r * g.out_stride + i] = v; }
     if (g.hit) g.hit[r * P + a] = 1;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Background randomisation, flip and normalisation of both images of each pair (the within-scene and across-scene
+// producers).  Per image a DDN_WS_PARAM_BYTES parameter block holds its decisions and colours (ddn_ws_batch_rand.params).
+//   total_a / total_b: mask totals at [pair * total_stride]; a pair whose total_a (or, when given, total_b) is 0 is the
+//     reference's return_empty_data: both outputs are the normalised, un-augmented image A.  total_a NULL: never empty.
+//   fmask (optional): the flipped masks [B, 2, P];  hit (optional): the matched-pixel bitmap [B, P], zeroed.
+struct AugmentArgs {
+  const uint8_t* rgb_a; const uint8_t* rgb_b; const uint8_t* mask_a; const uint8_t* mask_b;
+  const uint8_t* params; const uint8_t* noise;
+  const int* total_a; int64_t total_stride;
+  const int* total_b;
+  int randomize;
+  float* image_a; float* image_b; uint8_t* fmask; uint8_t* hit;
+  float mean[3], std[3];
+  int B, H, W;
+};
+
+// numpy.linspace(0, 1, n)[i]: i * (1 / (n - 1)), the last element exactly 1.0, [0.0] for n = 1
+__device__ __forceinline__ double linspace01(int i, int n) {
+  if (n < 2) return 0.0;
+  if (i == n - 1) return 1.0;
+  return __dmul_rn((double)i, __ddiv_rn(1.0, (double)(n - 1)));
+}
+
+// One thread per output pixel of image A or B of a pair.  The background randomisation (correspondence_augmentation.py:
+// 96-214) happens at the source pixel in the unflipped frame; the flip (ImageOps.flip + mirror) then reads that pixel for
+// the output pixel P-1-p; ToTensor + Normalize is ((x / 255) - mean) / std in fp32 with IEEE division.
+static __global__ void __launch_bounds__(256)
+augment_kernel(const AugmentArgs a) {
+  pdl_prologue();
+  const int64_t P = (int64_t)a.H * a.W, total = 2 * (int64_t)a.B * P;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t row = t / P, p = t - row * P, b = row >> 1;
+    const int img = (int)(row & 1);
+    const bool empty = a.total_a && (a.total_a[b * a.total_stride] == 0 || (a.total_b && a.total_b[b * a.total_stride] == 0));
+    const uint8_t* prm = a.params + row * DDN_WS_PARAM_BYTES;
+    const bool flip = !empty && prm[DDN_WS_FLIP];
+    const bool rnd = !empty && a.randomize && prm[DDN_WS_RANDOMIZE];
+    const int64_t q = flip ? P - 1 - p : p;
+    const bool src_a = img == 0 || empty;         // an empty pair returns image A twice
+    const uint8_t* rgb = (src_a ? a.rgb_a : a.rgb_b) + (b * P + q) * 3;
+    const int m = (src_a ? a.mask_a : a.mask_b)[b * P + q];
+    int v[3] = {rgb[0], rgb[1], rgb[2]};
+    if (rnd) {
+      const uint8_t* rgb1 = prm + DDN_WS_RGB1; const uint8_t* rgb2 = prm + DDN_WS_RGB2;
+      double pp = 0.0;
+      if (prm[DDN_WS_GRADIENT])
+        pp = prm[DDN_WS_VERTICAL] ? linspace01((int)(q / a.W), a.H) : linspace01((int)(q % a.W), a.W);
+      const uint8_t* n1 = a.noise + ((row * 2 + 0) * P + q) * 3;
+      const uint8_t* n2 = a.noise + ((row * 2 + 1) * P + q) * 3;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        // get_gradient_image: rgb2 * p + rgb1 * (1.0 - p) in fp64 (no FMA), truncated to uint8
+        int R = prm[DDN_WS_GRADIENT] ? (int)__dadd_rn(__dmul_rn((double)rgb2[c], pp), __dmul_rn((double)rgb1[c], __dsub_rn(1.0, pp)))
+                                     : (int)rgb1[c];
+        if (prm[DDN_WS_NOISE]) R += (int)n1[c] - (int)n2[c];
+        v[c] = (v[c] * m + ((1 - m) & 255) * (R & 255)) & 255;      // uint8 arithmetic modulo 256
+      }
+    }
+    float* out = (img == 0 ? a.image_a : a.image_b) + b * 3 * P + p;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c * P] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v[c], 255.f), a.mean[c]), a.std[c]);
+    if (a.fmask) a.fmask[row * P + p] = (uint8_t)m;
+    if (a.hit && img == 0) a.hit[b * P + p] = 0;
   }
 }
 

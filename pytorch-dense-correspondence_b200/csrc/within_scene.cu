@@ -10,11 +10,6 @@
 
 namespace ddn {
 
-struct NonzeroU8 {
-  const uint8_t* x; int64_t P;
-  __device__ __forceinline__ bool operator()(int64_t r, int64_t p) const { return x[r * P + p] != 0; }
-};
-
 // Row 3*pair + set over the flipped masks fmask [B, 2 (A, B), P] and the matched-pixel bitmap hit [B, P]:
 //   set 0: mask_b != 0 (masked non-matches, blind B side);  set 1: 1 - mask_b != 0 (background non-matches);
 //   set 2: mask_a - matched != 0 (blind A side, spartan_dataset_masked.py:736-739; an off-mask match gives -1 and is kept)
@@ -27,66 +22,6 @@ struct WsSets {
     return s == 0 ? m != 0 : m != 1;
   }
 };
-
-struct AugmentArgs {
-  const uint8_t* rgb_a; const uint8_t* rgb_b; const uint8_t* mask_a; const uint8_t* mask_b;
-  const uint8_t* params; const uint8_t* noise;
-  const int* total_a; int64_t total_stride;     // mask_a totals (empty pairs) when sampling on the mask, else NULL
-  int randomize;
-  float* image_a; float* image_b; uint8_t* fmask; uint8_t* hit;
-  float mean[3], std[3];
-  int B, H, W;
-};
-
-// numpy.linspace(0, 1, n)[i]: i * (1 / (n - 1)), the last element exactly 1.0, [0.0] for n = 1
-__device__ __forceinline__ double linspace01(int i, int n) {
-  if (n < 2) return 0.0;
-  if (i == n - 1) return 1.0;
-  return __dmul_rn((double)i, __ddiv_rn(1.0, (double)(n - 1)));
-}
-
-// One thread per output pixel of image A or B of a pair.  The background randomisation (correspondence_augmentation.py:
-// 96-214) happens at the source pixel in the unflipped frame; the flip (ImageOps.flip + mirror) then reads that pixel for
-// the output pixel P-1-p; ToTensor + Normalize is ((x / 255) - mean) / std in fp32 with IEEE division.
-__global__ void __launch_bounds__(256)
-augment_kernel(const AugmentArgs a) {
-  pdl_prologue();
-  const int64_t P = (int64_t)a.H * a.W, total = 2 * (int64_t)a.B * P;
-  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t row = t / P, p = t - row * P, b = row >> 1;
-    const int img = (int)(row & 1);
-    const bool empty = a.total_a && a.total_a[b * a.total_stride] == 0;
-    const uint8_t* prm = a.params + row * DDN_WS_PARAM_BYTES;
-    const bool flip = !empty && prm[DDN_WS_FLIP];
-    const bool rnd = !empty && a.randomize && prm[DDN_WS_RANDOMIZE];
-    const int64_t q = flip ? P - 1 - p : p;
-    const bool src_a = img == 0 || empty;         // an empty pair returns image A twice
-    const uint8_t* rgb = (src_a ? a.rgb_a : a.rgb_b) + (b * P + q) * 3;
-    const int m = (src_a ? a.mask_a : a.mask_b)[b * P + q];
-    int v[3] = {rgb[0], rgb[1], rgb[2]};
-    if (rnd) {
-      const uint8_t* rgb1 = prm + DDN_WS_RGB1; const uint8_t* rgb2 = prm + DDN_WS_RGB2;
-      double pp = 0.0;
-      if (prm[DDN_WS_GRADIENT])
-        pp = prm[DDN_WS_VERTICAL] ? linspace01((int)(q / a.W), a.H) : linspace01((int)(q % a.W), a.W);
-      const uint8_t* n1 = a.noise + ((row * 2 + 0) * P + q) * 3;
-      const uint8_t* n2 = a.noise + ((row * 2 + 1) * P + q) * 3;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        // get_gradient_image: rgb2 * p + rgb1 * (1.0 - p) in fp64 (no FMA), truncated to uint8
-        int R = prm[DDN_WS_GRADIENT] ? (int)__dadd_rn(__dmul_rn((double)rgb2[c], pp), __dmul_rn((double)rgb1[c], __dsub_rn(1.0, pp)))
-                                     : (int)rgb1[c];
-        if (prm[DDN_WS_NOISE]) R += (int)n1[c] - (int)n2[c];
-        v[c] = (v[c] * m + ((1 - m) & 255) * (R & 255)) & 255;      // uint8 arithmetic modulo 256
-      }
-    }
-    float* out = (img == 0 ? a.image_a : a.image_b) + b * 3 * P + p;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) out[c * P] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v[c], 255.f), a.mean[c]), a.std[c]);
-    a.fmask[row * P + p] = (uint8_t)m;
-    if (img == 0) a.hit[b * P + p] = 0;
-  }
-}
 
 struct BlindArgs {
   const int* nz3; const int* counts3; int64_t counts_stride; int nblk;   // rows 3*pair + set of the WsSets compaction
@@ -109,9 +44,7 @@ blind_kernel(const BlindArgs a) {
   const float* r = a.rand + b * P;
   for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < P; j += (int64_t)gridDim.x * blockDim.x) {
     if (j >= n) { out_a[j] = -1; out_b[j] = -1; continue; }
-    int q = (int)floorf(r[j] * (float)LB);
-    if (q >= LB) q = LB - 1;
-    out_a[j] = nz_a[j]; out_b[j] = nz_b[q];
+    out_a[j] = nz_a[j]; out_b[j] = masked_pick(r[j], LB, nz_b);
   }
 }
 
@@ -197,7 +130,7 @@ extern "C" int ddn_within_scene_batch(const ddn_ws_batch_cfg* cfg, const uint8_t
   const int* total_a = c.sample_matches_only_off_mask ? s.counts_a + nblkP : nullptr;
 
   // 2. background randomisation, flip and normalisation of both images; flipped masks; zeroed matched-pixel bitmap
-  AugmentArgs aug = {rgb_a, rgb_b, mask_a, mask_b, rand->params, rand->noise, total_a, csP, c.domain_randomize,
+  AugmentArgs aug = {rgb_a, rgb_b, mask_a, mask_b, rand->params, rand->noise, total_a, csP, nullptr, c.domain_randomize,
                      out->image_a, out->image_b, s.fmask, s.hit, {c.mean[0], c.mean[1], c.mean[2]},
                      {c.std[0], c.std[1], c.std[2]}, B, H, W};
   DDN_LAUNCH(augment_kernel, blocks(2 * B * P), 256, 0, st, aug);

@@ -1,6 +1,7 @@
 """Device-side non-match sampling (SURVEY.md 8f row 2): the index tensors ``loss_composer.get_loss`` consumes, produced on
 the GPU instead of by the CPU dataset workers (correspondence_finder.create_non_correspondences +
 SpartanDataset.create_non_matches + flatten_uv_tensor; see csrc/sampling.cu for the line references)."""
+import numpy as np
 import torch
 
 from . import _native as N
@@ -89,6 +90,19 @@ def _rand_shapes(B, H, W, c):
             "background_u": (B, n * c["k_background"]), "background_v": (B, n * c["k_background"]), "blind": (B, H * W)}
 
 
+def _rand_device(generator, device):
+    return torch.device(device) if device is not None else (generator.device if generator is not None else torch.device("cuda"))
+
+
+def _draw_augment_rand(B, H, W, generator, dev):
+    """``params`` and ``noise`` of the background randomisation and flip (the layout of draw_within_scene_rand)."""
+    params = torch.zeros(B, 2, N.WS_PARAM_BYTES, dtype=torch.uint8, device=dev)
+    params[:, :, :N.WS_RGB1] = torch.randint(0, 2, (B, 2, N.WS_RGB1), dtype=torch.uint8, device=dev, generator=generator)
+    params[:, :, N.WS_RGB1:N.WS_RGB2 + 3] = torch.randint(0, 255, (B, 2, 6), dtype=torch.uint8, device=dev, generator=generator)
+    return {"params": params,
+            "noise": torch.randint(0, 50, (B, 2, 2, H, W, 3), dtype=torch.uint8, device=dev, generator=generator)}
+
+
 def draw_within_scene_rand(B, H, W, training_config, generator=None, device=None):
     """Every random number ``within_scene_batch`` consumes for B pairs of H x W images, drawn on the device.
     -> dict: ``params`` uint8 [B, 2, 16] (image A, B: randomise / gradient / vertical / noise / flip decisions in {0, 1} at
@@ -96,12 +110,8 @@ def draw_within_scene_rand(B, H, W, training_config, generator=None, device=None
     [B, 2, 2, H, W, 3] in 0..49 (uint8(U * 50)), and the uniform fp32 arrays ``cand_u/v`` [B, n_attempts],
     ``masked_u/v`` [B, n_attempts * k_masked], ``background_u/v`` [B, n_attempts * k_background], ``blind`` [B, H * W]."""
     c = within_scene_cfg(training_config)
-    dev = torch.device(device) if device is not None else (generator.device if generator is not None else torch.device("cuda"))
-    params = torch.zeros(B, 2, N.WS_PARAM_BYTES, dtype=torch.uint8, device=dev)
-    params[:, :, :N.WS_RGB1] = torch.randint(0, 2, (B, 2, N.WS_RGB1), dtype=torch.uint8, device=dev, generator=generator)
-    params[:, :, N.WS_RGB1:N.WS_RGB2 + 3] = torch.randint(0, 255, (B, 2, 6), dtype=torch.uint8, device=dev, generator=generator)
-    out = {"params": params,
-           "noise": torch.randint(0, 50, (B, 2, 2, H, W, 3), dtype=torch.uint8, device=dev, generator=generator)}
+    dev = _rand_device(generator, device)
+    out = _draw_augment_rand(B, H, W, generator, dev)
     shapes = _rand_shapes(B, H, W, c)
     sizes = [shapes[k][0] * shapes[k][1] for k in _RAND_KEYS]
     flat = torch.rand(sum(sizes), device=dev, generator=generator)
@@ -184,4 +194,189 @@ def within_scene_batch(rgb_a, rgb_b, depth_a, depth_b, mask_a, mask_b, pose_a, p
     cnt = out["counts"].t().contiguous()
     out["num_valid"] = {"matches": cnt[0], "masked": cnt[1], "background": cnt[2], "blind": cnt[3]}
     out["match_type"] = torch.full((B,), SpartanDatasetDataType.SINGLE_OBJECT_WITHIN_SCENE, dtype=torch.int64)
+    return out
+
+
+# ----------------------------------------------------------------------------- across-scene training batches
+def across_scene_cfg(training_config):
+    """The ``training`` section of a training config -> the sizes of SpartanDataset.get_across_scene_data:
+    ``num_samples`` = cross_scene_num_samples (dense_correspondence_dataset_masked.py:549) and domain_randomize."""
+    t = training_config["training"]
+    return dict(num_samples=int(t["cross_scene_num_samples"]), domain_randomize=bool(t["domain_randomize"]))
+
+
+def draw_across_scene_rand(B, H, W, training_config, generator=None, device=None):
+    """Every random number ``across_scene_batch`` consumes for B pairs of H x W images, drawn on the device.
+    -> dict: ``params`` uint8 [B, 2, 16] and ``noise`` uint8 [B, 2, 2, H, W, 3] (as ``draw_within_scene_rand``), and the
+    uniform fp32 ``blind_a`` / ``blind_b`` [B, cross_scene_num_samples] (the draws over mask_a and mask_b)."""
+    n = across_scene_cfg(training_config)["num_samples"]
+    dev = _rand_device(generator, device)
+    out = _draw_augment_rand(B, H, W, generator, dev)
+    flat = torch.rand(2 * B * n, device=dev, generator=generator)
+    out["blind_a"], out["blind_b"] = flat[:B * n].view(B, n), flat[B * n:].view(B, n)
+    return out
+
+
+def across_scene_batch(rgb_a, rgb_b, mask_a, mask_b, training_config, generator=None, rand=None, match_type=None):
+    """SpartanDataset.get_across_scene_data (dataset/spartan_dataset_masked.py:1056-1141) for B image pairs on the device,
+    in one call that never synchronises with the host: the producer of DIFFERENT_OBJECT (get_different_object_data) and
+    SINGLE_OBJECT_ACROSS_SCENE (get_single_object_across_scene_data) pairs, which differ only in ``match_type``.
+
+    rgb_*: uint8 [B, H, W, 3]; mask_*: uint8 [B, H, W] (nonzero = object, any value); all CUDA.  The reference's depth
+    and poses only feed its debug plots and are not inputs.  ``training_config``: a config with the reference's
+    ``training`` section (cross_scene_num_samples, domain_randomize).  The random numbers are ``rand`` (as returned by
+    ``draw_across_scene_rand``) or are drawn from ``generator``.  ``match_type``: DIFFERENT_OBJECT (default) or
+    SINGLE_OBJECT_ACROSS_SCENE.
+    -> the keys of ``within_scene_batch``: ``image_a`` / ``image_b`` float32 [B, 3, H, W]; ``blind_non_matches_a/b`` int64
+    [B, cross_scene_num_samples]; ``matches_a/b``, ``masked_non_matches_a/b``, ``background_non_matches_a/b`` int64 [B, 0];
+    ``counts`` int64 [B, 4] (blind count in column 3); ``num_valid``; ``empty`` bool [B] (the reference's
+    return_empty_data: mask_a or mask_b empty; that pair's blind rows are -1 and both images are the normalised image A);
+    ``match_type`` (CPU)."""
+    import ctypes
+    from .loss_composer import SpartanDatasetDataType as T
+    if match_type is None:
+        match_type = T.DIFFERENT_OBJECT
+    if match_type not in (T.DIFFERENT_OBJECT, T.SINGLE_OBJECT_ACROSS_SCENE):
+        raise ValueError("across_scene_batch: match_type must be DIFFERENT_OBJECT or SINGLE_OBJECT_ACROSS_SCENE (got %r)"
+                         % (match_type,))
+    if training_config.get("training", {}).get("debug", False):
+        raise NotImplementedError("across_scene_batch: debug=True (plotting) is not supported")
+    c = across_scene_cfg(training_config)
+    if not isinstance(rgb_a, torch.Tensor) or rgb_a.dim() != 4:
+        raise RuntimeError("rgb_a must be a uint8 CUDA tensor [B, H, W, 3]")
+    B, H, W = rgb_a.shape[:3]
+    if not 1 <= B <= N.AS_MAX_PAIRS:
+        raise RuntimeError("across_scene_batch takes 1 to %d pairs per call (got %d)" % (N.AS_MAX_PAIRS, B))
+    dev = rgb_a.device
+    rgb_a = _require(rgb_a, "rgb_a", torch.uint8, (B, H, W, 3)); rgb_b = _require(rgb_b, "rgb_b", torch.uint8, (B, H, W, 3))
+    mask_a = _require(mask_a, "mask_a", torch.uint8, (B, H, W)); mask_b = _require(mask_b, "mask_b", torch.uint8, (B, H, W))
+    if rand is None:
+        rand = draw_across_scene_rand(B, H, W, training_config, generator=generator, device=dev)
+    n = c["num_samples"]
+    shapes = dict(params=(B, 2, N.WS_PARAM_BYTES), noise=(B, 2, 2, H, W, 3), blind_a=(B, n), blind_b=(B, n))
+    rand = {k: _require(rand[k], "rand[%r]" % k, torch.uint8 if k in ("params", "noise") else torch.float32, shapes[k])
+            for k in shapes}
+    i64 = dict(dtype=torch.int64, device=dev)
+    none = torch.empty(B, 0, **i64)
+    out = {"image_a": torch.empty(B, 3, H, W, device=dev), "image_b": torch.empty(B, 3, H, W, device=dev),
+           "matches_a": none, "matches_b": none.clone(), "masked_non_matches_a": none.clone(),
+           "masked_non_matches_b": none.clone(), "background_non_matches_a": none.clone(),
+           "background_non_matches_b": none.clone(),
+           "blind_non_matches_a": torch.empty(B, n, **i64), "blind_non_matches_b": torch.empty(B, n, **i64),
+           "counts": torch.empty(B, 4, **i64), "empty": torch.empty(B, dtype=torch.bool, device=dev)}
+    cfg = N.AsBatchCfg(B, H, W, int(c["domain_randomize"]), n, (ctypes.c_float * 3)(*IMAGE_MEAN), (ctypes.c_float * 3)(*IMAGE_STD))
+    r = N.AsBatchRand(*[rand[k].data_ptr() for k in ("params", "noise", "blind_a", "blind_b")])
+    o = N.AsBatchOut(*[out[k].data_ptr() for k in ("image_a", "image_b", "blind_non_matches_a", "blind_non_matches_b",
+                                                   "counts", "empty")])
+    nb = N.lib.ddn_across_scene_batch_scratch_bytes(ctypes.byref(cfg))
+    if nb == 0:
+        raise RuntimeError("across_scene_batch: configuration refused (%s, B=%d, H=%d, W=%d)" % (c, B, H, W))
+    scratch = torch.empty(nb, dtype=torch.uint8, device=dev)
+    N.check(N.lib.ddn_across_scene_batch(ctypes.byref(cfg), N.ptr(rgb_a), N.ptr(rgb_b), N.ptr(mask_a), N.ptr(mask_b),
+                                         ctypes.byref(r), ctypes.byref(o), N.ptr(scratch), nb, N.stream_ptr()))
+    cnt = out["counts"].t().contiguous()
+    out["num_valid"] = {"matches": cnt[0], "masked": cnt[1], "background": cnt[2], "blind": cnt[3]}
+    out["match_type"] = torch.full((B,), int(match_type), dtype=torch.int64)
+    return out
+
+
+# ----------------------------------------------------------------------------- synthetic multi-object training batches
+_SMO_RAND_KEYS = ("cand_u", "cand_v", "masked_u", "masked_v", "background_u", "background_v")
+
+
+def _smo_rand_shapes(B, c):
+    n = c["n_attempts"]
+    return {"cand_u": (B, 2, n), "cand_v": (B, 2, n), "masked_u": (B, 2 * n * c["k_masked"]),
+            "masked_v": (B, 2 * n * c["k_masked"]), "background_u": (B, 2 * n * c["k_background"]),
+            "background_v": (B, 2 * n * c["k_background"])}
+
+
+def draw_synthetic_multi_object_rand(B, H, W, training_config, generator=None, device=None):
+    """Every random number ``synthetic_multi_object_batch`` consumes for B pairs, drawn on the device.
+    -> dict: ``merge`` uint8 [B, 2] in {0, 1} (1: merge 1 / merge 2 puts scene B in the foreground, the reference's
+    ``random.random() < 0.5``), and the uniform fp32 ``cand_u/v`` [B, 2 (scene A, scene B), n_attempts],
+    ``masked_u/v`` [B, 2 * n_attempts * k_masked], ``background_u/v`` [B, 2 * n_attempts * k_background].  H and W are
+    accepted for symmetry with the other producers; no number depends on them."""
+    c = within_scene_cfg(training_config)
+    dev = _rand_device(generator, device)
+    out = {"merge": torch.randint(0, 2, (B, 2), dtype=torch.uint8, device=dev, generator=generator)}
+    shapes = _smo_rand_shapes(B, c)
+    sizes = [int(np.prod(shapes[k])) for k in _SMO_RAND_KEYS]
+    flat = torch.rand(sum(sizes), device=dev, generator=generator)
+    for k, part in zip(_SMO_RAND_KEYS, torch.split(flat, sizes)):
+        out[k] = part.view(shapes[k])
+    return out
+
+
+def synthetic_multi_object_batch(scene_a, scene_b, K, training_config, generator=None, rand=None):
+    """SpartanDataset.get_synthetic_multi_object_within_scene_data (dataset/spartan_dataset_masked.py:890-1053,
+    SYNTHETIC_MULTI_OBJECT) for B pairs on the device, in one call that never synchronises with the host.
+
+    scene_a, scene_b: 8-tuples ``(rgb_1, rgb_2, depth_1, depth_2, mask_1, mask_2, pose_1, pose_2)`` in
+    ``within_scene_batch``'s argument order: rgb uint8 [B, H, W, 3], depth float32 [B, H, W] (millimetres), mask uint8
+    [B, H, W] (CUDA); poses [B, 4, 4] camera-to-world on the host.  K: 3x3 intrinsics, shared by both scenes.  The random
+    numbers are ``rand`` (as returned by ``draw_synthetic_multi_object_rand``) or are drawn from ``generator``.
+    -> the keys of ``within_scene_batch``: ``image_a`` / ``image_b`` float32 [B, 3, H, W] (merged images 1 and 2);
+    ``matches_a/b`` [B, 2 * n_attempts], ``masked_non_matches_a/b`` [B, 2 * n_attempts * k_masked],
+    ``background_non_matches_a/b`` [B, 2 * n_attempts * k_background], ``blind_non_matches_a/b`` [B, 1] (always -1: the
+    reference returns empty_tensor()), int64 padded with -1; ``counts`` int64 [B, 4]; ``num_valid``; ``empty`` bool [B]
+    (one of the reference's four early returns); ``match_type`` (CPU, SYNTHETIC_MULTI_OBJECT).  At most 64 pairs per call:
+    each pair's two reprojection matrix sets travel as kernel parameters."""
+    import ctypes
+    from .loss_composer import SpartanDatasetDataType
+    if training_config.get("training", {}).get("debug", False):
+        raise NotImplementedError("synthetic_multi_object_batch: debug=True (plotting) is not supported")
+    c = within_scene_cfg(training_config)
+    if len(scene_a) != 8 or len(scene_b) != 8:
+        raise RuntimeError("scene_a / scene_b must be (rgb_1, rgb_2, depth_1, depth_2, mask_1, mask_2, pose_1, pose_2)")
+    if not isinstance(scene_a[0], torch.Tensor) or scene_a[0].dim() != 4:
+        raise RuntimeError("rgb_1 must be a uint8 CUDA tensor [B, H, W, 3]")
+    B, H, W = scene_a[0].shape[:3]
+    if not 1 <= B <= N.SMO_MAX_PAIRS:
+        raise RuntimeError("synthetic_multi_object_batch takes 1 to %d pairs per call (got %d)" % (N.SMO_MAX_PAIRS, B))
+    dev = scene_a[0].device
+    spec = (("rgb_1", torch.uint8, (B, H, W, 3)), ("rgb_2", torch.uint8, (B, H, W, 3)), ("depth_1", torch.float32, (B, H, W)),
+            ("depth_2", torch.float32, (B, H, W)), ("mask_1", torch.uint8, (B, H, W)), ("mask_2", torch.uint8, (B, H, W)))
+    stacked = {}
+    for i, (name, dt, shape) in enumerate(spec):
+        a = _require(scene_a[i], "scene_a." + name, dt, shape); b = _require(scene_b[i], "scene_b." + name, dt, shape)
+        stacked[name] = torch.stack((a, b), dim=1)              # [B, 2 (scene A, scene B), ...]
+    poses = {}
+    for i, name in ((6, "pose_1"), (7, "pose_2")):
+        pa = np.asarray(scene_a[i], dtype=np.float64); pb = np.asarray(scene_b[i], dtype=np.float64)
+        if pa.shape != (B, 4, 4) or pb.shape != (B, 4, 4):
+            raise RuntimeError("%s must have shape [B, 4, 4]" % name)
+        poses[name] = np.ascontiguousarray(np.stack((pa, pb), axis=1))
+    Kd = np.ascontiguousarray(np.asarray(K, dtype=np.float64).reshape(9))
+    if rand is None:
+        rand = draw_synthetic_multi_object_rand(B, H, W, training_config, generator=generator, device=dev)
+    shapes = dict(_smo_rand_shapes(B, c), merge=(B, 2))
+    rand = {k: _require(rand[k], "rand[%r]" % k, torch.uint8 if k == "merge" else torch.float32, shapes[k]) for k in shapes}
+    n = c["n_attempts"]
+    cap_m, cap_b = shapes["masked_u"][1], shapes["background_u"][1]
+    i64 = dict(dtype=torch.int64, device=dev)
+    out = {"image_a": torch.empty(B, 3, H, W, device=dev), "image_b": torch.empty(B, 3, H, W, device=dev),
+           "matches_a": torch.empty(B, 2 * n, **i64), "matches_b": torch.empty(B, 2 * n, **i64),
+           "masked_non_matches_a": torch.empty(B, cap_m, **i64), "masked_non_matches_b": torch.empty(B, cap_m, **i64),
+           "background_non_matches_a": torch.empty(B, cap_b, **i64), "background_non_matches_b": torch.empty(B, cap_b, **i64),
+           "blind_non_matches_a": torch.empty(B, 1, **i64), "blind_non_matches_b": torch.empty(B, 1, **i64),
+           "counts": torch.empty(B, 4, **i64), "empty": torch.empty(B, dtype=torch.bool, device=dev)}
+    cfg = N.SmoBatchCfg(B, H, W, int(c["sample_matches_only_off_mask"]), int(c["use_image_b_mask_inv"]), n, c["k_masked"],
+                        c["k_background"], (ctypes.c_float * 3)(*IMAGE_MEAN), (ctypes.c_float * 3)(*IMAGE_STD))
+    r = N.SmoBatchRand(*[rand[k].data_ptr() or None for k in ("merge",) + _SMO_RAND_KEYS])
+    o = N.SmoBatchOut(*[out[k].data_ptr() or None for k in (
+        "image_a", "image_b", "matches_a", "matches_b", "masked_non_matches_a", "masked_non_matches_b",
+        "background_non_matches_a", "background_non_matches_b", "blind_non_matches_a", "blind_non_matches_b", "counts", "empty")])
+    nb = N.lib.ddn_synthetic_multi_object_batch_scratch_bytes(ctypes.byref(cfg))
+    if nb == 0:
+        raise RuntimeError("synthetic_multi_object_batch: configuration refused (%s, B=%d, H=%d, W=%d)" % (c, B, H, W))
+    scratch = torch.empty(nb, dtype=torch.uint8, device=dev)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    N.check(N.lib.ddn_synthetic_multi_object_batch(
+        ctypes.byref(cfg), N.ptr(stacked["rgb_1"]), N.ptr(stacked["rgb_2"]), N.ptr(stacked["mask_1"]), N.ptr(stacked["mask_2"]),
+        N.ptr(stacked["depth_1"]), N.ptr(stacked["depth_2"]), vp(Kd), vp(poses["pose_1"]), vp(poses["pose_2"]),
+        ctypes.byref(r), ctypes.byref(o), N.ptr(scratch), nb, N.stream_ptr()))
+    cnt = out["counts"].t().contiguous()
+    out["num_valid"] = {"matches": cnt[0], "masked": cnt[1], "background": cnt[2], "blind": cnt[3]}
+    out["match_type"] = torch.full((B,), SpartanDatasetDataType.SYNTHETIC_MULTI_OBJECT, dtype=torch.int64)
     return out
