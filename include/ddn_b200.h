@@ -243,6 +243,31 @@ typedef struct {
 int ddn_within_scene_compose(const double* sums, const int64_t* counts, int B, int n_terms,
                              const ddn_within_scene_cfg* cfg_host, float* five, float* coef, void* stream);
 
+/* loss_composer.get_loss for a batch whose pairs have different SpartanDatasetDataType values: every pair gets its own
+ * type's formula, evaluated on the device from the sums/counts of the five terms
+ *   {match, masked, background, blind@M_masked, blind@M_background}
+ * (the last two read the same blind index tensors; the caller routes them with per-pair lengths: term 3 gets the blind
+ * count of the within-scene-type pairs and 0 for the others, term 4 the reverse).
+ *   SINGLE_OBJECT_WITHIN_SCENE, MULTI_OBJECT, SYNTHETIC_MULTI_OBJECT: get_within_scene_loss (loss_composer.py:70-143),
+ *     exactly as ddn_within_scene_compose with the blind term; the blind term is reported, never optimised.
+ *   DIFFERENT_OBJECT: get_different_object_loss (:168-191): blind = sum / max(#hard, 1) (scale_by_hard_negatives_
+ *     DIFFERENT_OBJECT) or sum / max(len_blind, 1); the pair's five values are (blind, 0, 0, 0, blind).
+ * pair_type [B] int32 DEVICE array; types are validated by the caller (SINGLE_OBJECT_ACROSS_SCENE has no loss upstream).
+ * five [5] fp32 = mean over B of the per-pair five values, summed in fp64 in a fixed order;
+ * coef [B, 5] fp32 = d(loss)/d(term sum), already divided by B.  n_terms must be 5. */
+typedef struct {
+  float match_loss_weight;
+  float non_match_loss_weight;
+  int32_t scale_by_hard_negatives;
+  int32_t scale_by_hard_negatives_different_object;
+  int64_t n_match, n_masked, n_background, n_blind;
+  /* per-pair true counts, DEVICE pointers [B] (NULL = the n_* above for every pair); len_blind is the unrouted blind count */
+  const int64_t* len_match; const int64_t* len_masked; const int64_t* len_background; const int64_t* len_blind;
+} ddn_pair_type_cfg;
+
+int ddn_pair_type_compose(const double* sums, const int64_t* counts, int B, int n_terms, const ddn_pair_type_cfg* cfg_host,
+                          const int32_t* pair_type, float* five, float* coef, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Host-buffer entry point (pageable or pinned host memory in, host memory out); it stages through
  * device memory it allocates itself and synchronises before returning.

@@ -44,6 +44,13 @@ class WithinSceneCfg(ctypes.Structure):
                 ("len_match", vp), ("len_masked", vp), ("len_background", vp), ("len_blind", vp)]
 
 
+class PairTypeComposeCfg(ctypes.Structure):
+    _fields_ = [("match_loss_weight", f32), ("non_match_loss_weight", f32),
+                ("scale_by_hard_negatives", ctypes.c_int32), ("scale_by_hard_negatives_different_object", ctypes.c_int32),
+                ("n_match", i64), ("n_masked", i64), ("n_background", i64), ("n_blind", i64),
+                ("len_match", vp), ("len_masked", vp), ("len_background", vp), ("len_blind", vp)]
+
+
 class WsBatchCfg(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32),
                 ("sample_matches_only_off_mask", ctypes.c_int32), ("domain_randomize", ctypes.c_int32),
@@ -129,6 +136,7 @@ _SIGNATURES = {
     "ddn_contrastive_terms_backward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32,
                                              vp, vp, vp, vp, vp]),
     "ddn_within_scene_compose": (i32, [vp, vp, i32, i32, ctypes.POINTER(WithinSceneCfg), vp, vp, vp]),
+    "ddn_pair_type_compose": (i32, [vp, vp, i32, i32, ctypes.POINTER(PairTypeComposeCfg), vp, vp, vp, vp]),
     "ddn_within_scene_loss_host": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, i64, vp, vp, i64, vp, vp, i64,
                                          f32, f32, f32, f32, i32, vp]),
     "ddn_conv2d_workspace_bytes": (sz, [i32] * 10),

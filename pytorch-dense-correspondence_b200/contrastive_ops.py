@@ -4,6 +4,8 @@
                           in the two descriptor images (used by every PixelwiseContrastiveLoss method).
 ``within_scene_loss``  -- fused loss_composer.get_within_scene_loss: one gather/reduce launch, one compose
                           launch, no host synchronisation; backward is one scatter launch.
+``pair_type_loss``     -- the same gather and scatter for a batch whose pairs have different SpartanDatasetDataType
+                          values (loss_composer.get_mixed_loss); the compose gives each pair its own type's loss.
 Descriptor images are consumed as the strided ``[B, P, D]`` views ``process_network_output`` makes.
 """
 import ctypes
@@ -129,29 +131,68 @@ def contrastive_terms(pred_a, pred_b, image_width, terms):
     return _Terms.apply(pred_a, pred_b, int(image_width), list(terms))
 
 
+def _within_scene_compose(sums, counts, cfg, five, coef, st):
+    B, T = sums.shape
+    N.check(N.lib.ddn_within_scene_compose(N.ptr(sums), N.ptr(counts), B, T, ctypes.byref(cfg), N.ptr(five), N.ptr(coef), st))
+
+
+def _pair_type_compose(sums, counts, cfg, five, coef, st):
+    B, T = sums.shape
+    N.check(N.lib.ddn_pair_type_compose(N.ptr(sums), N.ptr(counts), B, T, ctypes.byref(cfg), N.ptr(cfg._pair_type),
+                                        N.ptr(five), N.ptr(coef), st))
+
+
+def _fused_outputs(ctx, counts, five):
+    loss = five[0:1]
+    rest = five[1:].clone()
+    ctx.mark_non_differentiable(rest, counts)
+    return loss, rest, counts
+
+
+def _gather_compose(ctx, pred_a, pred_b, image_width, terms, cfg, compose):
+    """Forward of the fused losses from the full-resolution images: one gather launch, one ``compose`` launch."""
+    B, P, D = pred_a.shape
+    T = len(terms)
+    arr, keep = _build_terms(terms, B)
+    dev = pred_a.device
+    sums = torch.empty(B, T, dtype=torch.float64, device=dev)
+    counts = torch.empty(B, T, dtype=torch.int64, device=dev)
+    five = torch.empty(5, dtype=torch.float32, device=dev)
+    coef = torch.empty(B, T, dtype=torch.float32, device=dev)
+    sb, sp, sc = pred_a.stride()
+    st = N.stream_ptr()
+    N.check(N.lib.ddn_contrastive_terms_forward(N.ptr(pred_a), N.ptr(pred_b), sb, sp, sc, B, P, D, image_width,
+                                                arr, T, N.ptr(sums), N.ptr(counts), st))
+    compose(sums, counts, cfg, five, coef, st)
+    ctx.save_for_backward(pred_a, pred_b, coef)
+    ctx.arr, ctx.keep, ctx.image_width = arr, keep, image_width
+    return _fused_outputs(ctx, counts, five)
+
+
+def _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, compose):
+    """Forward of the fused losses through the bilinear upsample: one gather launch, one ``compose`` launch."""
+    B, _, D = low_a.shape
+    h, w, H, W = geom
+    T = len(terms)
+    arr, keep = _build_terms(terms, B)
+    dev = low_a.device
+    sums = torch.empty(B, T, dtype=torch.float64, device=dev)
+    counts = torch.empty(B, T, dtype=torch.int64, device=dev)
+    five = torch.empty(5, dtype=torch.float32, device=dev)
+    coef = torch.empty(B, T, dtype=torch.float32, device=dev)
+    st = N.stream_ptr()
+    N.check(N.lib.ddn_contrastive_terms_forward_lowres(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, arr, T,
+                                                       N.ptr(sums), N.ptr(counts), st))
+    compose(sums, counts, cfg, five, coef, st)
+    ctx.save_for_backward(low_a, low_b, coef)
+    ctx.arr, ctx.keep, ctx.geom = arr, keep, geom
+    return _fused_outputs(ctx, counts, five)
+
+
 class _WithinScene(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred_a, pred_b, image_width, terms, cfg):
-        B, P, D = pred_a.shape
-        T = len(terms)
-        arr, keep = _build_terms(terms, B)
-        dev = pred_a.device
-        sums = torch.empty(B, T, dtype=torch.float64, device=dev)
-        counts = torch.empty(B, T, dtype=torch.int64, device=dev)
-        five = torch.empty(5, dtype=torch.float32, device=dev)
-        coef = torch.empty(B, T, dtype=torch.float32, device=dev)
-        sb, sp, sc = pred_a.stride()
-        st = N.stream_ptr()
-        N.check(N.lib.ddn_contrastive_terms_forward(N.ptr(pred_a), N.ptr(pred_b), sb, sp, sc, B, P, D, image_width,
-                                                    arr, T, N.ptr(sums), N.ptr(counts), st))
-        N.check(N.lib.ddn_within_scene_compose(N.ptr(sums), N.ptr(counts), B, T, ctypes.byref(cfg), N.ptr(five),
-                                               N.ptr(coef), st))
-        ctx.save_for_backward(pred_a, pred_b, coef)
-        ctx.arr, ctx.keep, ctx.image_width = arr, keep, image_width
-        loss = five[0:1]
-        rest = five[1:].clone()
-        ctx.mark_non_differentiable(rest, counts)
-        return loss, rest, counts
+        return _gather_compose(ctx, pred_a, pred_b, image_width, terms, cfg, _within_scene_compose)
 
     @staticmethod
     def backward(ctx, dloss, _drest, _dcounts):
@@ -167,6 +208,15 @@ class _WithinScene(torch.autograd.Function):
         return da, db, None, None, None
 
 
+class _PairTypes(_WithinScene):
+    """The same gather and scatter as ``_WithinScene``; the compose gives every pair its own type's loss
+    (ddn_pair_type_compose)."""
+
+    @staticmethod
+    def forward(ctx, pred_a, pred_b, image_width, terms, cfg):
+        return _gather_compose(ctx, pred_a, pred_b, image_width, terms, cfg, _pair_type_compose)
+
+
 class _WithinSceneLowres(torch.autograd.Function):
     """within_scene_loss fused with the bilinear upsample: the descriptors are blended from the low-resolution maps
     ``low_a`` / ``low_b`` [B, h*w, D] (csrc/loss_lowres.cu); the gradient is scattered into d(low) -- the full-resolution
@@ -174,26 +224,7 @@ class _WithinSceneLowres(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, low_a, low_b, geom, terms, cfg):
-        B, _, D = low_a.shape
-        h, w, H, W = geom
-        T = len(terms)
-        arr, keep = _build_terms(terms, B)
-        dev = low_a.device
-        sums = torch.empty(B, T, dtype=torch.float64, device=dev)
-        counts = torch.empty(B, T, dtype=torch.int64, device=dev)
-        five = torch.empty(5, dtype=torch.float32, device=dev)
-        coef = torch.empty(B, T, dtype=torch.float32, device=dev)
-        st = N.stream_ptr()
-        N.check(N.lib.ddn_contrastive_terms_forward_lowres(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, arr, T,
-                                                           N.ptr(sums), N.ptr(counts), st))
-        N.check(N.lib.ddn_within_scene_compose(N.ptr(sums), N.ptr(counts), B, T, ctypes.byref(cfg), N.ptr(five),
-                                               N.ptr(coef), st))
-        ctx.save_for_backward(low_a, low_b, coef)
-        ctx.arr, ctx.keep, ctx.geom = arr, keep, geom
-        loss = five[0:1]
-        rest = five[1:].clone()
-        ctx.mark_non_differentiable(rest, counts)
-        return loss, rest, counts
+        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _within_scene_compose)
 
     @staticmethod
     def backward(ctx, dloss, _drest, _dcounts):
@@ -208,6 +239,14 @@ class _WithinSceneLowres(torch.autograd.Function):
                                                             N.ptr(coef), N.ptr(up), N.ptr(da), N.ptr(db), N.ptr(scratch),
                                                             N.stream_ptr()))
         return da, db, None, None, None
+
+
+class _PairTypesLowres(_WithinSceneLowres):
+    """``_PairTypes`` through the bilinear upsample (the gather and scatter of ``_WithinSceneLowres``)."""
+
+    @staticmethod
+    def forward(ctx, low_a, low_b, geom, terms, cfg):
+        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _pair_type_compose)
 
 
 def within_scene_loss(pred_a, pred_b, image_width, terms, match_loss_weight, non_match_loss_weight,
@@ -233,3 +272,34 @@ def within_scene_loss(pred_a, pred_b, image_width, terms, match_loss_weight, non
         low_a, low_b, geom = lowres
         return _WithinSceneLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg)
     return _WithinScene.apply(pred_a, pred_b, int(image_width), list(terms), cfg)
+
+
+def pair_type_loss(pred_a, pred_b, image_width, terms, pair_type, match_loss_weight, non_match_loss_weight,
+                   scale_by_hard_negatives, scale_by_hard_negatives_different_object, lengths, lowres=None):
+    """terms = [match, masked, background, blind@M_masked, blind@M_background], the two blind terms over the same index
+    tensors with their lengths routed by pair type; pair_type: [B] int32 CUDA SpartanDatasetDataType values; lengths =
+    (matches, masked, background, blind) [B] int64 CUDA true counts (blind unrouted).  -> as ``within_scene_loss``: every
+    pair scored by its own type's formula, mean over the B pairs; only ``loss`` carries gradient."""
+    pred_a = _as_pred(pred_a, "image_a_pred")
+    pred_b = _strides(pred_a, _as_pred(pred_b, "image_b_pred"))
+    B = pred_a.shape[0]
+    if len(terms) != 5:
+        raise RuntimeError("pair_type_loss takes 5 terms (got %d)" % len(terms))
+    if not isinstance(pair_type, torch.Tensor) or not pair_type.is_cuda or pair_type.dtype != torch.int32 \
+            or pair_type.shape != (B,):
+        raise RuntimeError("pair_type must be a CUDA int32 tensor of shape [%d]" % B)
+    n = [_as_index(t.idx_a, B, "indices").shape[1] for t in terms]
+    cfg = N.PairTypeComposeCfg(float(match_loss_weight), float(non_match_loss_weight), int(bool(scale_by_hard_negatives)),
+                               int(bool(scale_by_hard_negatives_different_object)), n[0], n[1], n[2], n[3])
+    keep = [pair_type]
+    for field, t in zip(("len_match", "len_masked", "len_background", "len_blind"), lengths):
+        t = _as_lengths(t, B, field)
+        if t is None:
+            raise RuntimeError("pair_type_loss needs every per-pair count (%s is missing)" % field)
+        keep.append(t)
+        setattr(cfg, field, t.data_ptr())
+    cfg._keep, cfg._pair_type = keep, pair_type.contiguous()
+    if lowres is not None:
+        low_a, low_b, geom = lowres
+        return _PairTypesLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg)
+    return _PairTypes.apply(pred_a, pred_b, int(image_width), list(terms), cfg)

@@ -228,6 +228,67 @@ __global__ void within_scene_compose_kernel(const double* __restrict__ sums, con
   }
 }
 
+// SpartanDatasetDataType.DIFFERENT_OBJECT (dataset/spartan_dataset_masked.py:31-36); every other type the caller lets
+// through is a within-scene type.
+constexpr int PAIR_DIFFERENT_OBJECT = 2;
+
+// Terms {match, masked, background, blind@M_masked, blind@M_background}.  Each pair takes its own type's formula:
+// within-scene types as within_scene_compose_kernel with the blind term (loss_composer.py:70-143), DIFFERENT_OBJECT
+// loss_composer.py:168-191.  One warp, lane-strided over pairs, then a fixed-order warp sum, as the kernel above.
+__global__ void pair_type_compose_kernel(const double* __restrict__ sums, const unsigned long long* __restrict__ counts,
+                                         int B, ddn_pair_type_cfg cfg, const int32_t* __restrict__ pair_type,
+                                         float* __restrict__ five, float* __restrict__ coef) {
+  pdl_prologue();
+  constexpr int NT = 5;
+  double acc[5] = {0, 0, 0, 0, 0};
+  for (int b = threadIdx.x; b < B; b += 32) {
+    const double* S = sums + b * NT;
+    const unsigned long long* H = counts + b * NT;
+    float* cf = coef + b * NT;
+    if (pair_type[b] == PAIR_DIFFERENT_OBJECT) {
+      long long n;
+      if (cfg.scale_by_hard_negatives_different_object) n = (long long)H[4];
+      else n = cfg.len_blind ? (long long)cfg.len_blind[b] : (long long)cfg.n_blind;
+      const double scale = (double)(n > 1 ? n : 1);
+      const double blind = S[4] / scale;
+      acc[0] += blind; acc[4] += blind;
+      cf[0] = cf[1] = cf[2] = cf[3] = 0.f;
+      cf[4] = (float)(1.0 / (scale * B));
+      continue;
+    }
+    const long long n_match = cfg.len_match ? (long long)cfg.len_match[b] : (long long)cfg.n_match;
+    double match = S[0] / (double)(n_match > 1 ? n_match : 1);
+    double Sm = S[1], Sb = S[2], Sx = S[3];
+    double scale, tm, tb, tx;
+    if (cfg.scale_by_hard_negatives) {
+      long long hm = (long long)H[1], hb = (long long)H[2], hx = (long long)H[3];
+      long long tot = hm + hb; if (tot < 1) tot = 1;
+      scale = (double)tot;
+      tm = Sm / (double)(hm > 1 ? hm : 1);
+      tb = Sb / (double)(hb > 1 ? hb : 1);
+      tx = Sx / (double)(hx > 1 ? hx : 1);
+    } else {
+      long long nm = cfg.len_masked ? (long long)cfg.len_masked[b] : (long long)cfg.n_masked;
+      long long nb = cfg.len_background ? (long long)cfg.len_background[b] : (long long)cfg.n_background;
+      long long nx = cfg.len_blind ? (long long)cfg.len_blind[b] : (long long)cfg.n_blind;
+      nm = nm > 1 ? nm : 1; nb = nb > 1 ? nb : 1; nx = nx > 1 ? nx : 1;
+      scale = (double)(nm + nb);
+      tm = Sm / (double)nm; tb = Sb / (double)nb; tx = Sx / (double)nx;
+    }
+    double non_match = (Sm + Sb) / scale;
+    double loss = cfg.match_loss_weight * match + cfg.non_match_loss_weight * non_match;
+    acc[0] += loss; acc[1] += match; acc[2] += tm; acc[3] += tb; acc[4] += tx;
+    cf[0] = (float)(cfg.match_loss_weight / ((double)(n_match > 1 ? n_match : 1) * B));
+    cf[1] = cf[2] = (float)(cfg.non_match_loss_weight / (scale * B));
+    cf[3] = cf[4] = 0.f;   // blind non-matches of a within-scene pair are reported, never optimised
+  }
+#pragma unroll
+  for (int i = 0; i < 5; ++i) {
+    double v = warp_sum(acc[i]);
+    if (threadIdx.x == 0) five[i] = (float)(v / B);
+  }
+}
+
 __global__ void scale_inplace_kernel(float* __restrict__ g, int64_t n, float s) {
   pdl_prologue();
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -310,6 +371,16 @@ extern "C" int ddn_within_scene_compose(const double* sums, const int64_t* count
   DDN_CHECK_ARG(cfg->n_match > 0, "n_match must be positive");
   DDN_LAUNCH(within_scene_compose_kernel, 1, 32, 0, (cudaStream_t)stream, sums,
              reinterpret_cast<const unsigned long long*>(counts), B, n_terms, *cfg, five, coef);
+  return 0;
+}
+
+extern "C" int ddn_pair_type_compose(const double* sums, const int64_t* counts, int B, int n_terms,
+                                     const ddn_pair_type_cfg* cfg, const int32_t* pair_type, float* five, float* coef,
+                                     void* stream) {
+  DDN_CHECK_ARG(sums && counts && cfg && pair_type && five && coef, "null argument");
+  DDN_CHECK_ARG(B >= 1 && n_terms == 5, "pair-type compose needs B >= 1 and 5 terms");
+  DDN_LAUNCH(pair_type_compose_kernel, 1, 32, 0, (cudaStream_t)stream, sums,
+             reinterpret_cast<const unsigned long long*>(counts), B, *cfg, pair_type, five, coef);
   return 0;
 }
 

@@ -8,12 +8,13 @@ loss_composer.py:107-141 on the device, and the backward is ONE scatter kernel.
 
 Batch extension (the reference is batch-1 only, training.py:314-323): descriptor images may be
 ``[B, W*H, D]`` with ``[B, n]`` index tensors; the loss is then the mean over the B pairs of the reference's
-per-pair loss (SURVEY.md 8a).
+per-pair loss (SURVEY.md 8a).  ``get_loss`` keeps the reference's rule that all pairs of a call share one type;
+``get_mixed_loss`` (opt-in) scores a batch of mixed types, each pair by its own type's loss.
 """
 import torch
 
 from . import _native as N
-from .contrastive_ops import Term, within_scene_loss, contrastive_terms
+from .contrastive_ops import Term, within_scene_loss, contrastive_terms, pair_type_loss
 from .resnet_dilated import lowres_of
 
 
@@ -94,6 +95,67 @@ def get_loss(pixelwise_contrastive_loss, match_type,
         return get_different_object_loss(pixelwise_contrastive_loss, image_a_pred, image_b_pred,
                                          blind_non_matches_a, blind_non_matches_b)
     raise ValueError("Should only have above scenes?")
+
+
+_NUM_VALID_KEYS = ("matches", "masked", "background", "blind")
+
+
+def get_mixed_loss(pixelwise_contrastive_loss, match_type,
+                   image_a_pred, image_b_pred,
+                   matches_a, matches_b,
+                   masked_non_matches_a, masked_non_matches_b,
+                   background_non_matches_a, background_non_matches_b,
+                   blind_non_matches_a, blind_non_matches_b, num_valid):
+    """``get_loss`` for a batch whose pairs have different types, as the reference would score them one sample at a time:
+    each pair gets its own type's loss -- ``get_within_scene_loss`` for SINGLE_OBJECT_WITHIN_SCENE, MULTI_OBJECT and
+    SYNTHETIC_MULTI_OBJECT, ``get_different_object_loss`` for DIFFERENT_OBJECT -- and the five values are the means over the
+    B pairs (a uniform batch gives what ``get_loss`` gives).  One gather launch, one compose launch, one scatter launch in
+    the backward, and no host synchronisation.
+
+    ``match_type``: the CPU ``[B]`` tensor the producers return (``sampling.concat_batches`` for a mixed batch), checked on
+    the host; ``num_valid``: the producers' dict of ``[B]`` int64 CUDA per-pair counts (required).  Only ``loss`` carries
+    gradient.  A SINGLE_OBJECT_ACROSS_SCENE pair raises the NameError the reference's loss raises for that type."""
+    T = SpartanDatasetDataType
+    mt = torch.as_tensor(match_type)
+    if mt.is_cuda or mt.dim() != 1 or mt.numel() < 1 or mt.is_floating_point():
+        raise ValueError("match_type must be a CPU integer tensor of shape [B]")
+    known = torch.tensor([T.SINGLE_OBJECT_WITHIN_SCENE, T.SINGLE_OBJECT_ACROSS_SCENE, T.DIFFERENT_OBJECT, T.MULTI_OBJECT,
+                          T.SYNTHETIC_MULTI_OBJECT])
+    if not bool(torch.isin(mt, known).all()):
+        raise ValueError("Should only have above scenes?")
+    if bool((mt == T.SINGLE_OBJECT_ACROSS_SCENE).any()):
+        raise NameError("name 'pcl' is not defined")         # get_same_object_across_scene_loss, loss_composer.py:203
+    if num_valid is None or any(num_valid.get(k) is None for k in _NUM_VALID_KEYS):
+        raise ValueError("get_mixed_loss needs num_valid with the per-pair counts %s" % (_NUM_VALID_KEYS,))
+    pcl = pixelwise_contrastive_loss
+    cfg = pcl._config
+    dev = image_a_pred.device
+    pair_type = mt.to(torch.int32).pin_memory().to(dev, non_blocking=True)
+    blind = num_valid["blind"]
+    different = pair_type == T.DIFFERENT_OBJECT
+    blind_within, blind_different = torch.where(different, 0, blind), torch.where(different, blind, 0)
+    # different-object pairs have no matches, so the pixel-distance weighting only ever reaches within-scene pairs; a batch
+    # with no match column at all has nothing to weight
+    has_matches = matches_b.shape[-1] > 0
+    gt_m = matches_b if cfg["use_l2_pixel_loss_on_masked_non_matches"] and has_matches else None
+    gt_b = matches_b if cfg["use_l2_pixel_loss_on_background_non_matches"] and has_matches else None
+    terms = [
+        Term(matches_a, matches_b, N.TERM_MATCH, lengths=num_valid["matches"]),
+        Term(masked_non_matches_a, masked_non_matches_b, N.TERM_HINGE, cfg["M_masked"], gt_b=gt_m,
+             m_pixel=cfg["M_pixel"], lengths=num_valid["masked"], gt_lengths=num_valid["matches"]),
+        Term(background_non_matches_a, background_non_matches_b, N.TERM_HINGE, cfg["M_background"], gt_b=gt_b,
+             m_pixel=cfg["M_pixel"], lengths=num_valid["background"], gt_lengths=num_valid["matches"]),
+        Term(blind_non_matches_a, blind_non_matches_b, N.TERM_HINGE, cfg["M_masked"], lengths=blind_within),
+        Term(blind_non_matches_a, blind_non_matches_b, N.TERM_HINGE, cfg["M_background"], lengths=blind_different),
+    ]
+    loss, rest, counts = pair_type_loss(image_a_pred, image_b_pred, pcl.image_width, terms, pair_type,
+                                        cfg["match_loss_weight"], cfg["non_match_loss_weight"],
+                                        cfg["scale_by_hard_negatives"], cfg["scale_by_hard_negatives_DIFFERENT_OBJECT"],
+                                        tuple(num_valid[k] for k in _NUM_VALID_KEYS),
+                                        lowres=_fused_lowres(image_a_pred, image_b_pred, pcl.image_width))
+    if pcl.debug:
+        pcl.debug_data["num_hard_negatives_device"] = counts
+    return loss, rest[0:1], rest[1:2], rest[2:3], rest[3:4]
 
 
 def get_within_scene_loss(pixelwise_contrastive_loss, image_a_pred, image_b_pred,

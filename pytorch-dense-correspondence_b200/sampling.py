@@ -280,6 +280,91 @@ def across_scene_batch(rgb_a, rgb_b, mask_a, mask_b, training_config, generator=
     return out
 
 
+# ----------------------------------------------------------------------------- mixed pair-type batches
+# The order in which SpartanDataset lists the types it draws from (dense_correspondence_dataset_masked.py:557-586)
+DATA_TYPE_ORDER = ("SINGLE_OBJECT_WITHIN_SCENE", "SINGLE_OBJECT_ACROSS_SCENE", "DIFFERENT_OBJECT", "MULTI_OBJECT",
+                   "SYNTHETIC_MULTI_OBJECT")
+INDEX_KEYS = ("matches_a", "matches_b", "masked_non_matches_a", "masked_non_matches_b", "background_non_matches_a",
+              "background_non_matches_b", "blind_non_matches_a", "blind_non_matches_b")
+
+
+def draw_data_types(B, training_config, generator=None):
+    """One SpartanDatasetDataType per pair, drawn as SpartanDataset draws one per sample (_get_data_load_type,
+    dense_correspondence_dataset_masked.py:557-586 and np.random.choice): the types of
+    ``training.data_type_probabilities`` with p > 0, in the reference's order, probabilities normalised, each pair drawn
+    independently (uniform u, first type whose cumulative probability exceeds u).  ``generator``: a CPU torch.Generator,
+    so a seed gives the same types on every machine.  -> CPU int64 [B]."""
+    from .loss_composer import SpartanDatasetDataType
+    probs = training_config.get("training", {}).get("data_type_probabilities")
+    if probs is None:
+        raise ValueError("training_config has no training.data_type_probabilities")
+    if isinstance(B, bool) or not isinstance(B, int) or B < 1:
+        raise ValueError("B must be a positive int (got %r)" % (B,))
+    if generator is not None and generator.device.type != "cpu":
+        raise ValueError("draw_data_types draws with a CPU torch.Generator (got one on %s)" % generator.device)
+    types, p = [], []
+    for name in DATA_TYPE_ORDER:
+        if name not in probs:
+            raise ValueError("data_type_probabilities has no %s" % name)
+        v = float(probs[name])
+        if not v >= 0.0 or v == float("inf"):
+            raise ValueError("data_type_probabilities[%s] must be finite and >= 0 (got %r)" % (name, probs[name]))
+        if v > 0:
+            types.append(getattr(SpartanDatasetDataType, name))
+            p.append(v)
+    if not p:
+        raise ValueError("every data_type_probabilities entry is 0")
+    cdf = torch.tensor(p, dtype=torch.float64).cumsum(0)
+    cdf /= cdf[-1].clone()
+    u = torch.rand(B, dtype=torch.float64, generator=generator)
+    idx = torch.searchsorted(cdf, u, right=True).clamp_(max=len(p) - 1)
+    return torch.tensor(types, dtype=torch.int64)[idx]
+
+
+def concat_batches(parts):
+    """One batch from several producer outputs (``within_scene_batch``, ``across_scene_batch``,
+    ``synthetic_multi_object_batch``, any ``match_type`` relabelling kept), pairs in part order: the images concatenated,
+    each index key padded with -1 to the widest part then concatenated, ``counts``, ``empty`` and ``match_type``
+    concatenated and ``num_valid`` rebuilt from ``counts``.  Pair order does not change the loss or the BatchNorm
+    statistics, so no shuffle is needed.  Everything stays on the device without a host synchronisation; the number of
+    launches depends on the number of parts, not on B."""
+    if not parts:
+        raise ValueError("concat_batches needs at least one part")
+    shape = tuple(parts[0]["image_a"].shape[1:])
+    match_types = []
+    for i, p in enumerate(parts):
+        if tuple(p["image_a"].shape[1:]) != shape or tuple(p["image_b"].shape[1:]) != shape:
+            raise ValueError("concat_batches: every part must have images of shape [B, %s]" % ", ".join(map(str, shape)))
+        mt = torch.as_tensor(p["match_type"])
+        if mt.device.type != "cpu":      # the types are checked and read on the host (get_mixed_loss), without a sync
+            raise ValueError("concat_batches: match_type of part %d is on %s; keep it the CPU tensor the producers return "
+                             "(relabel with torch.full_like(out[\"match_type\"], t))" % (i, mt.device))
+        if tuple(mt.shape) != (p["image_a"].shape[0],):
+            raise ValueError("concat_batches: match_type of part %d must have shape [%d] (got %s)"
+                             % (i, p["image_a"].shape[0], tuple(mt.shape)))
+        match_types.append(mt.to(torch.int64))
+    rows = [p["image_a"].shape[0] for p in parts]
+    dev = parts[0]["image_a"].device
+    out = {"image_a": torch.cat([p["image_a"] for p in parts]), "image_b": torch.cat([p["image_b"] for p in parts])}
+    for k in INDEX_KEYS:
+        width = max(p[k].shape[1] for p in parts)
+        t = torch.empty(sum(rows), width, dtype=torch.int64, device=dev)
+        r = 0
+        for p, n in zip(parts, rows):
+            w = p[k].shape[1]
+            t[r:r + n, :w].copy_(p[k])
+            if w < width:
+                t[r:r + n, w:].fill_(-1)
+            r += n
+        out[k] = t
+    out["counts"] = torch.cat([p["counts"] for p in parts])
+    out["empty"] = torch.cat([p["empty"] for p in parts])
+    out["match_type"] = torch.cat(match_types)
+    cnt = out["counts"].t().contiguous()
+    out["num_valid"] = {"matches": cnt[0], "masked": cnt[1], "background": cnt[2], "blind": cnt[3]}
+    return out
+
+
 # ----------------------------------------------------------------------------- synthetic multi-object training batches
 _SMO_RAND_KEYS = ("cand_u", "cand_v", "masked_u", "masked_v", "background_u", "background_v")
 

@@ -4,8 +4,10 @@ RGB images and flat pixel indices n = u + W*v (doc/coordinate_conventions.md), w
 ``non_matches_a`` being every match repeated k times consecutively (spartan_dataset_masked.py:853-854).
 
 Pure CPU torch with an explicit generator, so the same call reproduces the same tensors in the
-build container and on the GPU box (SURVEY.md section 8d).
+build container and on the GPU box (SURVEY.md section 8d).  ``plane_scene_pairs`` gives the raw inputs of the device
+batch producers in ``sampling`` (uint8 RGB, masks, depth in millimetres, camera poses) for a ray-cast plane.
 """
+import numpy as np
 import torch
 
 
@@ -37,3 +39,43 @@ def make_pair_batch(B, H=480, W=640, num_matches=1000, num_masked=1000, num_back
     out["background_a"], out["background_b"] = non_matches(num_background)
     out["blind_a"], out["blind_b"] = non_matches(num_blind)
     return out
+
+
+def plane_scene_pairs(B, H, W, seed, empty=()):
+    """B image pairs of a ray-cast tilted plane seen from two nearby camera poses, with random RGB and blob masks: the
+    inputs of ``sampling.within_scene_batch`` / ``across_scene_batch`` / ``synthetic_multi_object_batch`` (one scene).
+    mask_a of the pairs whose index is in ``empty`` is all zero (every producer's return_empty_data).
+    -> (dict of CPU tensors ``rgb_a/b`` uint8 [B, H, W, 3], ``depth_a/b`` float32 [B, H, W] (millimetres), ``mask_a/b``
+    uint8 [B, H, W], and numpy ``pose_a/b`` [B, 4, 4] camera-to-world; K, the 3x3 intrinsics scaled from 640x480)."""
+    K = np.array([[533.6422696034836 * W / 640, 0, 319.4091030774892 * W / 640], [0, 534.7824445233571 * H / 480,
+                  236.4374299691866 * H / 480], [0, 0, 1.0]])
+    g = np.random.RandomState(seed)
+
+    def pose(rx, ry, t):
+        cx, sx, cy, sy = np.cos(rx), np.sin(rx), np.cos(ry), np.sin(ry)
+        Rx = np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]); Ry = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
+        T4 = np.eye(4); T4[:3, :3] = Ry.dot(Rx); T4[:3, 3] = t
+        return T4
+
+    us, vs = np.meshgrid(np.arange(W), np.arange(H))
+    rays = np.linalg.inv(K).dot(np.stack([us.ravel(), vs.ravel(), np.ones(H * W)]))
+
+    def render(T4):
+        nrm, d0 = np.array([-0.1, 0.05, 1.0]), 1.2
+        s = (d0 - nrm.dot(T4[:3, 3])) / nrm.dot(T4[:3, :3].dot(rays))
+        return np.round(s * 1000.0).reshape(H, W).astype(np.float32)
+
+    x = {k: [] for k in ("rgb_a", "rgb_b", "depth_a", "depth_b", "mask_a", "mask_b", "pose_a", "pose_b")}
+    for b in range(B):
+        pa = pose(0.02 * g.randn(), 0.02 * g.randn(), [0, 0, 0]); pb = pose(0.05 * g.randn(), 0.1 * g.randn(), 0.05 * g.randn(3))
+        mask_a = (g.rand(H, W) > 0.1).astype(np.uint8); mask_a[: H // 4] = 0
+        mask_b = (g.rand(H, W) > 0.2).astype(np.uint8); mask_b[:, : W // 3] = 0
+        if b in empty:
+            mask_a[:] = 0
+        for k, v in (("rgb_a", g.randint(0, 256, (H, W, 3))), ("rgb_b", g.randint(0, 256, (H, W, 3))),
+                     ("depth_a", render(pa)), ("depth_b", render(pb)), ("mask_a", mask_a), ("mask_b", mask_b),
+                     ("pose_a", pa), ("pose_b", pb)):
+            x[k].append(v)
+    dt = dict(rgb_a=torch.uint8, rgb_b=torch.uint8, depth_a=torch.float32, depth_b=torch.float32, mask_a=torch.uint8,
+              mask_b=torch.uint8)
+    return {k: torch.from_numpy(np.stack(v)).to(dt[k]) if k in dt else np.stack(v) for k, v in x.items()}, K
