@@ -442,6 +442,43 @@ int ddn_match_statistics(const float* res_a, const int64_t* strides_a_host, cons
                          float* out_f32, double* out_f64, int64_t* out_i64, int64_t* bad_queries,
                          void* scratch, size_t scratch_bytes, void* stream);
 
+/* Best match of Q query pixels over N image pairs in one launch: the across-object analysis
+ * (compute_descriptor_match_statistics_no_ground_truth, dense_correspondence/evaluation/evaluation.py:977-1004), i.e.
+ * find_best_match (dense_correspondence_network.py:488-525) of uv_a[q] in res_a[pair[q]] against all of res_b[pair[q]].
+ *   res_a/b, strides_*_host, N, H, W, D   as ddn_match_statistics (1 <= D <= 32, element strides over (n, h, w, c))
+ *   pair [Q] int64, uv_a [Q,2] int64 (u, v)   DEVICE
+ * Outputs: best_uv [Q,2] int64 (u, v) and best_diff [Q] float32, the distance nd at it, computed as ddn_match_statistics
+ * computes nd (bit-equal to numpy on a contiguous array); ties go to the first pixel in row-major order (np.argmin).  A
+ * query whose pair or uv_a is out of range gets (-1, -1) and NaN and is counted in *bad_queries (DEVICE int64,
+ * overwritten).  The result does not depend on the order in which blocks run: a second call is bit-identical.
+ * scratch: ddn_best_match_batch_scratch_bytes(Q) bytes (0 for Q outside 1..DDN_BM_MAX_QUERIES). */
+#define DDN_BM_MAX_QUERIES (65535 * 8)
+size_t ddn_best_match_batch_scratch_bytes(int64_t Q);
+int ddn_best_match_batch(const float* res_a, const int64_t* strides_a_host, const float* res_b, const int64_t* strides_b_host,
+                         int N, int H, int W, int D, const int64_t* pair, const int64_t* uv_a, int64_t Q,
+                         int64_t* best_uv, float* best_diff, int64_t* bad_queries, void* scratch, size_t scratch_bytes,
+                         void* stream);
+
+/* Per-image, per-channel descriptor statistics in one launch: the body of compute_descriptor_statistics
+ * (dense_correspondence/evaluation/evaluation.py:2177-2219) for N images at once.
+ *   res            N descriptor images, element (n, h, w, c) at res[n*s[0] + h*s[1] + w*s[2] + c*s[3]] with
+ *                  s = strides_host [4] (HOST int64, elements): the NCHW network output and the [H,W,D] view of
+ *                  forward_single_image_tensor both work without a copy.  1 <= D <= 32.
+ *   mask           [N,H,W] contiguous DEVICE, DDN_DS_MASK_F32 (float32) or DDN_DS_MASK_U8 (uint8); nonzero = object.
+ * Outputs (DEVICE): out_stats [N, DDN_DS_NSTATS, D] float32 in the order of DDN_DS_* below; out_count [N] int64, the
+ * nonzero mask pixels.  min / max propagate NaN as torch.min / torch.max do; means are fp64 sums over the pixels (per
+ * block, then the blocks in a fixed order by the image's last block), divided by the count and rounded once to float32,
+ * so a second call is bit-identical.  An empty mask gives count 0 and NaN mask statistics; nothing is raised.
+ * scratch: ddn_descriptor_statistics_scratch_bytes(N, H, W, D) bytes (0 for sizes outside the limits). */
+enum { DDN_DS_MASK_F32 = 0, DDN_DS_MASK_U8 = 1 };
+enum { DDN_DS_MIN = 0, DDN_DS_MAX = 1, DDN_DS_MEAN = 2, DDN_DS_MASK_MIN = 3, DDN_DS_MASK_MAX = 4, DDN_DS_MASK_MEAN = 5,
+       DDN_DS_NSTATS = 6 };
+#define DDN_DS_MAX_IMAGES 65535
+size_t ddn_descriptor_statistics_scratch_bytes(int N, int H, int W, int D);
+int ddn_descriptor_statistics(const float* res, const int64_t* strides_host, int N, int H, int W, int D, const void* mask,
+                              int mask_dtype, float* out_stats, int64_t* out_count, void* scratch, size_t scratch_bytes,
+                              void* stream);
+
 /* Non-match sampling on the device: out_b[j] = flat index (u + W*v) of a pixel drawn uniformly from the nonzero pixels of
  * `mask` [H*W] fp32 (nz[floor(rand_u[j] * #nonzero)], nonzero pixels in ascending order) or, when mask is NULL or empty,
  * from the whole image (floor(rand_u*W), floor(rand_v*H)); out_a[j] = matches_a[j / non_matches_per_match] (may be NULL).

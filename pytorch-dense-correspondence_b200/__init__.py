@@ -14,8 +14,10 @@ from . import loss_composer
 from .loss_composer import SpartanDatasetDataType
 from .fused_adam import FusedAdam, adjust_learning_rate
 from . import ops, synthetic, data_parallel, sampling, evaluation
-from .evaluation import DenseCorrespondenceEvaluation, match_statistics, quantitative_analysis_on_pair
+from .evaluation import (DenseCorrespondenceEvaluation, match_statistics, quantitative_analysis_on_pair, descriptor_statistics,
+                         descriptor_statistics_over_images, save_descriptor_statistics, across_object_analysis)
 
 __all__ = ["Resnet34_8s", "Resnet50_8s", "DenseCorrespondenceNetwork", "PixelwiseContrastiveLoss", "loss_composer",
            "SpartanDatasetDataType", "DEFAULT_LOSS_CONFIG", "set_default_precision", "FusedAdam", "adjust_learning_rate", "ops", "synthetic", "data_parallel", "sampling",
-           "evaluation", "DenseCorrespondenceEvaluation", "match_statistics", "quantitative_analysis_on_pair"]
+           "evaluation", "DenseCorrespondenceEvaluation", "match_statistics", "quantitative_analysis_on_pair",
+           "descriptor_statistics", "descriptor_statistics_over_images", "save_descriptor_statistics", "across_object_analysis"]

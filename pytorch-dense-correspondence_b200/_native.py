@@ -172,6 +172,10 @@ _SIGNATURES = {
     "ddn_match_statistics_scratch_bytes": (sz, [i32, i32, i32, i64]),
     "ddn_match_statistics": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
                                    vp, sz, vp]),
+    "ddn_best_match_batch_scratch_bytes": (sz, [i64]),
+    "ddn_best_match_batch": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, i64, vp, vp, vp, vp, sz, vp]),
+    "ddn_descriptor_statistics_scratch_bytes": (sz, [i32, i32, i32, i32]),
+    "ddn_descriptor_statistics": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, vp, vp, vp, sz, vp]),
     "ddn_adam_step": (i32, [vp, vp, vp, vp, i64, i64, f32, f32, f32, f32, f32, f32, vp]),
     "ddn_profile_enable": (i32, [i32]),
     "ddn_profile_reset": (i32, []),

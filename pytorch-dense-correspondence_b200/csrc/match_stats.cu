@@ -9,6 +9,10 @@
 // match_stats_finish_kernel: one thread per query adds its partial records in block order (so a second call is
 //   bit-identical) and writes the reference's columns.
 // L2/load bound like best_match_kernel; MS_GROUP queries read the image once instead of MS_GROUP times.
+// best_match_batch_kernel: the same scan with the best match only, for the across-object analysis
+//   (compute_descriptor_match_statistics_no_ground_truth, evaluation.py:977-1004): per block a 64-bit atomicMax of the
+//   complemented key (order-independent, so deterministic), and the last block of each query group (bn_stats.cuh's
+//   ticket) writes (u, v) and the distance.  One launch for every pair and query.
 //
 // Arithmetic, as the reference's numpy does it on a contiguous [H,W,D] float32 array (net.py:488-525):
 //   nd(p) = sqrt(sum_c (res_b[p,c] - q_c)^2): each square rounded before it is added (no FMA), the sum in numpy's float32
@@ -18,6 +22,7 @@
 #include <climits>
 #include <cmath>
 #include <initializer_list>
+#include "bn_stats.cuh"
 #include "common.cuh"
 
 namespace ddn {
@@ -89,6 +94,34 @@ __device__ __forceinline__ void ms_load(const MsImage& im, int64_t n, int64_t v,
   for (int c = 0; c < KD; ++c) x[c] = c < D ? __ldg(p + c * im.sc) : 0.f;
 }
 
+// The full-image best-match scan (find_best_match, net.py:488-525) shared by every kernel here: each of this thread's
+// pixels p in [p0, p1) is scored against the group's valid queries, and visit(j, p, v, u, nd, m) receives query j's
+// distance nd(p) and, with MASK, mask_b at p (0 otherwise).  When the group's queries share an image pair (`uni`) a
+// pixel's descriptor (and mask value) is loaded once for all of them.
+template <int KD, bool MASK, typename Visit>
+__device__ __forceinline__ void ms_scan_pixels(const MsImage& rb, const float* __restrict__ mask_b, int64_t P, int W, int D,
+                                               int64_t p0, int64_t p1, const float (*qd)[KD], const int64_t* qn,
+                                               const int* qok, bool uni, Visit&& visit) {
+  for (int64_t p = p0 + threadIdx.x; p < p1; p += MS_THREADS) {
+    const int64_t v = p / W, u = p - v * W;
+    float x[KD];
+    float m = 0.f;
+    if (uni) {
+      ms_load<KD>(rb, qn[0], v, u, D, x);
+      if (MASK) m = __ldg(mask_b + qn[0] * P + p);
+    }
+#pragma unroll
+    for (int j = 0; j < MS_GROUP; ++j) {
+      if (!qok[j]) continue;
+      if (!uni) {
+        ms_load<KD>(rb, qn[j], v, u, D, x);
+        if (MASK) m = __ldg(mask_b + qn[j] * P + p);
+      }
+      visit(j, p, v, u, ms_norm_diff<KD>(x, qd[j], D), m);
+    }
+  }
+}
+
 template <int KD>
 __global__ void __launch_bounds__(MS_THREADS)
 match_stats_scan_kernel(MsImage ra, MsImage rb, int N, int H, int W, int D,
@@ -139,37 +172,22 @@ match_stats_scan_kernel(MsImage ra, MsImage rb, int N, int H, int W, int D,
   for (int j = 0; j < MS_GROUP; ++j) {
     key[j] = ~0ull; mval[j] = INFINITY; midx[j] = INT_MAX; cnt[j] = cntm[j] = mcnt[j] = 0; sum[j] = summ[j] = 0.0;
   }
-  for (int64_t p = p0 + threadIdx.x; p < p1; p += MS_THREADS) {
-    const int64_t v = p / W, u = p - v * W;
-    float x[KD];
-    float m = 0.f;
-    if (uni) {
-      ms_load<KD>(rb, qn[0], v, u, D, x);
-      m = __ldg(mask_b + qn[0] * P + p);
+  ms_scan_pixels<KD, true>(rb, mask_b, P, W, D, p0, p1, qd, qn, qok, uni,
+                           [&](int j, int64_t p, int64_t v, int64_t u, float nd, float m) {
+    const unsigned long long k = ((unsigned long long)__float_as_uint(nd) << 32) | (unsigned long long)(uint32_t)p;
+    key[j] = k < key[j] ? k : key[j];
+    const double md = __dadd_rn((double)nd, __dmul_rn(__dsub_rn(1.0, (double)m), 1e6));
+    if (md < mval[j]) { mval[j] = md; midx[j] = (int)p; }      // pixels rise along a thread: strict < keeps the first
+    const float t = thr[j];
+    const bool c1 = nd < t, c2 = md < (double)t;
+    if (c1 || c2) {
+      const int64_t du = u - qub[j], dv = v - qvb[j];
+      const double dist = __dsqrt_rn((double)(du * du + dv * dv));
+      if (c1) { cnt[j] += 1; sum[j] = __dadd_rn(sum[j], dist); }
+      if (c2) { cntm[j] += 1; summ[j] = __dadd_rn(summ[j], dist); }
     }
-#pragma unroll
-    for (int j = 0; j < MS_GROUP; ++j) {
-      if (!qok[j]) continue;
-      if (!uni) {
-        ms_load<KD>(rb, qn[j], v, u, D, x);
-        m = __ldg(mask_b + qn[j] * P + p);
-      }
-      const float nd = ms_norm_diff<KD>(x, qd[j], D);
-      const unsigned long long k = ((unsigned long long)__float_as_uint(nd) << 32) | (unsigned long long)(uint32_t)p;
-      key[j] = k < key[j] ? k : key[j];
-      const double md = __dadd_rn((double)nd, __dmul_rn(__dsub_rn(1.0, (double)m), 1e6));
-      if (md < mval[j]) { mval[j] = md; midx[j] = (int)p; }      // pixels rise along a thread: strict < keeps the first
-      const float t = thr[j];
-      const bool c1 = nd < t, c2 = md < (double)t;
-      if (c1 || c2) {
-        const int64_t du = u - qub[j], dv = v - qvb[j];
-        const double dist = __dsqrt_rn((double)(du * du + dv * dv));
-        if (c1) { cnt[j] += 1; sum[j] = __dadd_rn(sum[j], dist); }
-        if (c2) { cntm[j] += 1; summ[j] = __dadd_rn(summ[j], dist); }
-      }
-      mcnt[j] += m != 0.f;
-    }
-  }
+    mcnt[j] += m != 0.f;
+  });
 
   // block reduction in a fixed order: xor-shuffle tree inside each warp, then the warps in index order
   __shared__ MsPartial red[MS_THREADS / 32][MS_GROUP];
@@ -309,6 +327,89 @@ __global__ void match_stats_finish_kernel(const MsPartial* __restrict__ part, in
   i64[DDN_MS_NUM_CLOSER] = r.cnt; i64[DDN_MS_NUM_CLOSER_MASKED] = r.cntm; i64[DDN_MS_NUM_MASK_PIXELS] = r.mcnt;
 }
 
+// best[q] holds ~key (zero on entry: no candidate yet), ticket[group] zero on entry; both are left as the caller zeroed them
+// except that the tickets return to zero.  A query whose pair or pixel is out of range gets (-1, -1), NaN and is counted.
+template <int KD>
+__global__ void __launch_bounds__(MS_THREADS)
+best_match_batch_kernel(MsImage ra, MsImage rb, int N, int H, int W, int D, const int64_t* __restrict__ pair,
+                        const int64_t* __restrict__ uv_a, int64_t Q, int pixels_per_block, unsigned long long* __restrict__ best,
+                        unsigned int* __restrict__ ticket, int64_t* __restrict__ out_uv, float* __restrict__ out_diff,
+                        unsigned long long* __restrict__ bad) {
+  pdl_prologue();
+  __shared__ float qd[MS_GROUP][KD];
+  __shared__ int64_t qn[MS_GROUP];
+  __shared__ int qok[MS_GROUP];
+  __shared__ int uniform, last;
+  const int64_t q0 = (int64_t)blockIdx.y * MS_GROUP;
+  if (threadIdx.x < MS_GROUP) {
+    const int j = threadIdx.x;
+    const int64_t q = q0 + j;
+    int ok = 0;
+    if (q < Q) {
+      const int64_t n = pair[q], ua = uv_a[2 * q], va = uv_a[2 * q + 1];
+      ok = ms_query_ok(n, ua, va, 0, 0, N, H, W);
+      if (ok) {
+        float x[KD];
+        ms_load<KD>(ra, n, va, ua, D, x);
+#pragma unroll
+        for (int c = 0; c < KD; ++c) qd[j][c] = x[c];
+        qn[j] = n;
+      }
+    }
+    qok[j] = ok;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int u = qok[0];
+    for (int j = 1; j < MS_GROUP; ++j) u &= (!qok[j] || qn[j] == qn[0]);
+    uniform = u;
+  }
+  __syncthreads();
+  const int64_t P = (int64_t)H * W;
+  const int64_t p0 = (int64_t)blockIdx.x * pixels_per_block;
+  const int64_t p1 = min(P, p0 + pixels_per_block);
+  unsigned long long key[MS_GROUP];
+#pragma unroll
+  for (int j = 0; j < MS_GROUP; ++j) key[j] = ~0ull;
+  ms_scan_pixels<KD, false>(rb, nullptr, P, W, D, p0, p1, qd, qn, qok, uniform != 0,
+                            [&](int j, int64_t p, int64_t, int64_t, float nd, float) {
+    const unsigned long long k = ((unsigned long long)__float_as_uint(nd) << 32) | (unsigned long long)(uint32_t)p;
+    key[j] = k < key[j] ? k : key[j];
+  });
+  __shared__ unsigned long long red[MS_THREADS / 32][MS_GROUP];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int j = 0; j < MS_GROUP; ++j) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long other = __shfl_xor_sync(0xffffffffu, key[j], o);
+      key[j] = other < key[j] ? other : key[j];
+    }
+    if (lane == 0) red[warp][j] = key[j];
+  }
+  __syncthreads();
+  if (threadIdx.x < MS_GROUP && qok[threadIdx.x]) {
+    unsigned long long k = red[0][threadIdx.x];
+    for (int w = 1; w < MS_THREADS / 32; ++w) k = red[w][threadIdx.x] < k ? red[w][threadIdx.x] : k;
+    if (k != ~0ull) atomicMax(best + q0 + threadIdx.x, ~k);
+  }
+  if (!bn_last_cta(ticket + blockIdx.y, gridDim.x, threadIdx.x == 0, &last, [] { __syncthreads(); })) return;
+  if (threadIdx.x < MS_GROUP) {
+    const int64_t q = q0 + threadIdx.x;
+    if (q >= Q) return;
+    if (!qok[threadIdx.x]) {
+      out_uv[2 * q] = -1; out_uv[2 * q + 1] = -1; out_diff[q] = NAN;
+      atomicAdd(bad, 1ull);
+      return;
+    }
+    const unsigned long long k = ~__ldcg(best + q);
+    const uint32_t p = (uint32_t)(k & 0xffffffffull);
+    out_uv[2 * q] = p % W;          // u = column
+    out_uv[2 * q + 1] = p / W;      // v = row
+    out_diff[q] = __uint_as_float((uint32_t)(k >> 32));
+  }
+}
+
 // The pixel split depends on H*W alone, so the scratch size needs no device query.
 static int ms_blocks_x(int64_t P, int* ppb) {
   int nb = (int)std::min<int64_t>(64, std::max<int64_t>(1, ceil_div(P, 4096)));
@@ -386,5 +487,68 @@ extern "C" int ddn_match_statistics(const float* res_a, const int64_t* strides_a
     DDN_LAUNCH(match_stats_scan_kernel<32>, grid, MS_THREADS, 0, st, ia, ib, N, H, W, D, pair, uv_a, uv_b, Q, mask_b, ppb, part);
   DDN_LAUNCH(match_stats_finish_kernel, (unsigned)ceil_div(Q, 128), 128, 0, st, part, nb, N, H, W, pair, uv_a, uv_b, Q, depth_a,
              depth_b, ki, poses, poses + 16 * N, out_f32, out_f64, out_i64, reinterpret_cast<unsigned long long*>(bad_queries));
+  return 0;
+}
+
+static bool bm_sizes_ok(int N, int H, int W, int64_t Q) {
+  return N >= 1 && N <= DDN_MS_MAX_PAIRS && H >= 1 && W >= 1 && (int64_t)H * W < (1ll << 31) && Q >= 1 &&
+         Q <= DDN_BM_MAX_QUERIES;
+}
+
+// [groups * MS_GROUP] complemented keys, then [groups] tickets
+static size_t bm_scratch_bytes(int64_t Q) {
+  const int64_t groups = ceil_div(Q, MS_GROUP);
+  return sizeof(unsigned long long) * (size_t)(groups * MS_GROUP) + align_up(sizeof(unsigned int) * (size_t)groups, 256);
+}
+
+extern "C" size_t ddn_best_match_batch_scratch_bytes(int64_t Q) {
+  if (Q < 1 || Q > DDN_BM_MAX_QUERIES) {
+    set_error("ddn_best_match_batch_scratch_bytes: Q %lld outside 1..%d", (long long)Q, DDN_BM_MAX_QUERIES);
+    return 0;
+  }
+  return bm_scratch_bytes(Q);
+}
+
+extern "C" int ddn_best_match_batch(const float* res_a, const int64_t* strides_a_host, const float* res_b,
+                                    const int64_t* strides_b_host, int N, int H, int W, int D, const int64_t* pair,
+                                    const int64_t* uv_a, int64_t Q, int64_t* best_uv, float* best_diff, int64_t* bad_queries,
+                                    void* scratch, size_t scratch_bytes, void* stream) {
+  DDN_CHECK_ARG(res_a && res_b && strides_a_host && strides_b_host && pair && uv_a && best_uv && best_diff && bad_queries &&
+                scratch, "ddn_best_match_batch: null argument");
+  DDN_CHECK_ARG(D >= 1 && D <= MS_MAXD, "ddn_best_match_batch: descriptor dimension %d outside 1..%d", D, MS_MAXD);
+  DDN_CHECK_ARG(bm_sizes_ok(N, H, W, Q), "ddn_best_match_batch: bad sizes (N %d in 1..%d, H*W < 2^31, Q %lld in 1..%d)", N,
+                DDN_MS_MAX_PAIRS, (long long)Q, DDN_BM_MAX_QUERIES);
+  const int64_t ext[4] = {N, H, W, D};
+  for (const int64_t* s : {strides_a_host, strides_b_host}) {
+    int64_t last = 0;
+    for (int i = 0; i < 4; ++i) {
+      DDN_CHECK_ARG(s[i] >= 0 && s[i] < (1ll << 40), "ddn_best_match_batch: stride %lld out of range", (long long)s[i]);
+      last += (ext[i] - 1) * s[i];
+    }
+    DDN_CHECK_ARG(last < (1ll << 40), "ddn_best_match_batch: strides address more than 2^40 elements");
+  }
+  DDN_CHECK_ARG(scratch_bytes >= bm_scratch_bytes(Q), "ddn_best_match_batch: scratch %zu < %zu bytes", scratch_bytes,
+                bm_scratch_bytes(Q));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t groups = ceil_div(Q, MS_GROUP);
+  unsigned long long* best = reinterpret_cast<unsigned long long*>(scratch);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(best + groups * MS_GROUP);
+  DDN_CUDA(cudaMemsetAsync(scratch, 0, bm_scratch_bytes(Q), st));
+  DDN_CUDA(cudaMemsetAsync(bad_queries, 0, sizeof(int64_t), st));
+  const MsImage ia{res_a, strides_a_host[0], strides_a_host[1], strides_a_host[2], strides_a_host[3]};
+  const MsImage ib{res_b, strides_b_host[0], strides_b_host[1], strides_b_host[2], strides_b_host[3]};
+  int ppb;
+  const int nb = ms_blocks_x((int64_t)H * W, &ppb);
+  dim3 grid(nb, (unsigned)groups);
+  unsigned long long* bad = reinterpret_cast<unsigned long long*>(bad_queries);
+  if (D <= 8)
+    DDN_LAUNCH(best_match_batch_kernel<8>, grid, MS_THREADS, 0, st, ia, ib, N, H, W, D, pair, uv_a, Q, ppb, best, ticket, best_uv,
+               best_diff, bad);
+  else if (D <= 16)
+    DDN_LAUNCH(best_match_batch_kernel<16>, grid, MS_THREADS, 0, st, ia, ib, N, H, W, D, pair, uv_a, Q, ppb, best, ticket, best_uv,
+               best_diff, bad);
+  else
+    DDN_LAUNCH(best_match_batch_kernel<32>, grid, MS_THREADS, 0, st, ia, ib, N, H, W, D, pair, uv_a, Q, ppb, best, ticket, best_uv,
+               best_diff, bad);
   return 0;
 }

@@ -4,9 +4,9 @@ running in libddn_b200.so.
 
 Kept verbatim in behaviour: ``forward`` (:239-263), ``forward_single_image_tensor`` (:265-299),
 ``process_network_output`` (:303-319), ``get_fcn`` (:360-383), ``from_config`` (:386-438),
-``from_model_folder`` (:441-485), ``find_best_match`` (:488-525) and the properties training.py /
-evaluation.py read.  Left out (not on the hot path, need the dataset stack / PIL / utils module):
-``load_training_dataset``, ``descriptor_image_stats``, ``get_unet`` -- they raise NotImplementedError.
+``from_model_folder`` (:441-485), ``find_best_match`` (:488-525), ``descriptor_image_stats`` (:136-152) and the
+properties training.py / evaluation.py read.  Left out (not on the hot path, need the dataset stack / PIL / utils
+module): ``load_training_dataset``, ``get_unet`` -- they raise NotImplementedError.
 """
 import logging
 import os
@@ -91,7 +91,16 @@ class DenseCorrespondenceNetwork(nn.Module):
 
     @property
     def descriptor_image_stats(self):
-        raise NotImplementedError("descriptor statistics live in the evaluation stack (out of scope, SURVEY.md 2a #7)")
+        """net.py:136-152: descriptor_statistics.yaml of the network's parameter folder (written by
+        evaluation.save_descriptor_statistics), loaded on first use.  A relative folder is taken relative to the home
+        directory, as utils.convert_to_absolute_path does."""
+        if self._descriptor_image_stats is None:
+            path = self.path_to_network_params_folder
+            if not os.path.isdir(path):
+                path = os.path.join(os.path.expanduser("~"), path)
+            with open(os.path.join(path, "descriptor_statistics.yaml")) as f:
+                self._descriptor_image_stats = yaml.safe_load(f)
+        return self._descriptor_image_stats
 
     def load_training_dataset(self):
         raise NotImplementedError("the SpartanDataset stack is out of scope (SURVEY.md 2a #5)")

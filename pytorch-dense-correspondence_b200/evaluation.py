@@ -7,6 +7,12 @@ records for each ground-truth match, for many matches over many image pairs in o
 ``quantitative_analysis_on_pair`` is the dataset-free body of ``single_same_scene_image_pair_quantitative_analysis``
 (evaluation.py:862-958).
 
+Two further steps of ``run_evaluation_on_network`` (evaluation.py:2308-2410) that need no dataset stack:
+``descriptor_statistics`` / ``descriptor_statistics_over_images`` / ``save_descriptor_statistics`` compute and write
+descriptor_statistics.yaml (``compute_descriptor_statistics_on_dataset``, :2157-2305; csrc/descriptor_stats.cu), which
+``DenseCorrespondenceNetwork.descriptor_image_stats`` reads back; ``best_match_batch`` / ``across_object_analysis`` are
+the across-object analysis (``evaluate_network_across_objects``, :305-338, 784-858, 977-1004) in one best-match launch.
+
 Reference quirks that are kept: the depth at uv_a is never checked for validity (evaluation.py:1103); ``compute_3d_position``
 is called with (u, v) although its docstring says (row, column) (:1112-1115, :1185); an empty mask_b divides by an integer
 zero (:1086), which the batched call reports as a NaN fraction and ``compute_descriptor_match_statistics`` as
@@ -257,3 +263,222 @@ def quantitative_analysis_on_pair(dcn, rgb_a, rgb_b, depth_a, depth_b, mask_a, m
     rows = {k: v.cpu().numpy() for k, v in out.items() if k != "bad_queries"}
     rows["uv_a"] = uv_a.cpu().numpy(); rows["uv_b"] = uv_b.cpu().numpy()
     return rows
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Descriptor statistics (compute_descriptor_statistics_on_dataset, evaluation.py:2157-2305; csrc/descriptor_stats.cu)
+
+STAT_KEYS = ['min', 'max', 'mean', 'mask_min', 'mask_max', 'mask_mean']      # row order of ddn_descriptor_statistics
+
+
+def descriptor_statistics(res, mask):
+    """Per-image, per-channel descriptor statistics of N images in one launch (compute_descriptor_statistics,
+    evaluation.py:2177-2219).
+
+    res   [N,H,W,D] (or [H,W,D]) float32 CUDA, any strides: pass the network's NCHW output as ``res.permute(0, 2, 3, 1)``
+          and forward_single_image_tensor's [H,W,D] view as it is; neither is copied.  1 <= D <= 32.
+    mask  [N,H,W] (or [H,W]) CUDA float32, uint8 or bool; nonzero = object.
+    -> {'min', 'max', 'mean', 'mask_min', 'mask_max', 'mask_mean': [N,D] float32, 'mask_count': [N] int64} CUDA tensors,
+    without a host synchronisation.  Whole-image statistics use every pixel, mask statistics the nonzero mask pixels; an
+    image with an empty mask has mask_count 0 and NaN mask statistics.  min / max are torch.min / torch.max exactly;
+    means are fp64 sums rounded once to float32 (torch's float32 mean may differ from them in the last bits)."""
+    if not isinstance(res, torch.Tensor) or not res.is_cuda:
+        raise RuntimeError("res must be a CUDA tensor: this path has no CPU fallback")
+    N.require_cuda_f32(res, "res", contiguous=False)
+    res = _batched(res, "res", 4)
+    n, H, W, D = res.shape
+    if not 1 <= D <= MAX_D:
+        raise RuntimeError("descriptor dimension %d outside 1..%d" % (D, MAX_D))
+    mask = _batched(mask, "mask", 3, device=res.device)
+    if tuple(mask.shape) != (n, H, W):
+        raise RuntimeError("mask must have shape %s (got %s)" % ((n, H, W), tuple(mask.shape)))
+    if mask.dtype == torch.bool:
+        mask = mask.view(torch.uint8)
+    if mask.dtype not in (torch.float32, torch.uint8):
+        raise RuntimeError("mask must be float32, uint8 or bool (got %s)" % mask.dtype)
+    mask = mask.contiguous()
+    dev = res.device
+    stats = torch.empty(n, len(STAT_KEYS), D, dtype=torch.float32, device=dev)
+    count = torch.empty(n, dtype=torch.int64, device=dev)
+    nb = N.lib.ddn_descriptor_statistics_scratch_bytes(n, H, W, D)
+    if nb == 0:
+        raise N.DdnError(N.lib.ddn_last_error().decode())
+    scratch = torch.empty(nb, dtype=torch.uint8, device=dev)
+    strides = np.array(res.stride(), dtype=np.int64)
+    N.check(N.lib.ddn_descriptor_statistics(N.ptr(res), strides.ctypes.data_as(ctypes.c_void_p), n, H, W, D, N.ptr(mask),
+                                            0 if mask.dtype == torch.float32 else 1, N.ptr(stats), N.ptr(count), N.ptr(scratch),
+                                            nb, N.stream_ptr()))
+    out = {k: stats[:, i] for i, k in enumerate(STAT_KEYS)}
+    out['mask_count'] = count
+    return out
+
+
+def fold_descriptor_statistics(per_image, num_images=None):
+    """update_stats and the final loop of compute_descriptor_statistics_on_dataset (evaluation.py:2237-2292) over
+    per-image statistics ({key: [N,D]} and 'mask_count' [N], as descriptor_statistics returns them; tensors or arrays).
+
+    Reference quirks kept: an image whose mask is empty is skipped for both keys (:2279-2282); the mean is the float32 sum
+    of the kept images' means times 1/num_images (num_images defaults to N, the images asked for, even when some were
+    skipped; :2290); if every image was skipped the reference fails with a TypeError (None * float), and so does this.
+    -> {'entire_image': {'mean', 'max', 'min': [D] lists}, 'mask_image': {...}}, the schema of descriptor_statistics.yaml."""
+    host = {k: (v.cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)) for k, v in per_image.items()}
+    n = host['mask_count'].shape[0]
+    num_images = n if num_images is None else int(num_images)
+    stats = {'entire_image': {'mean': None, 'max': None, 'min': None}, 'mask_image': {'mean': None, 'max': None, 'min': None}}
+    for i in range(n):
+        if host['mask_count'][i] == 0:
+            continue
+        for key, prefix in (('entire_image', ''), ('mask_image', 'mask_')):
+            d = stats[key]
+            mn, mx, mean = (np.asarray(host[prefix + s][i], dtype=np.float32) for s in ('min', 'max', 'mean'))
+            # torch.min / torch.max of two tensors, like np.minimum / np.maximum, propagate NaN
+            d['min'] = mn.copy() if d['min'] is None else np.minimum(d['min'], mn)
+            d['max'] = mx.copy() if d['max'] is None else np.maximum(d['max'], mx)
+            d['mean'] = mean.copy() if d['mean'] is None else d['mean'] + mean          # float32 += float32
+    for key, val in stats.items():
+        if val['mean'] is None:
+            raise TypeError("every mask was empty: compute_descriptor_statistics_on_dataset fails here too "
+                            "(1.0/num_images * None, evaluation.py:2290)")
+        val['mean'] = np.float32(1.0 / num_images) * val['mean']       # a float32 tensor times a Python float
+        for field in val:
+            val[field] = [float(x) for x in val[field]]
+    return stats
+
+
+def descriptor_statistics_over_images(dcn, rgbs, masks):
+    """The dataset-free body of compute_descriptor_statistics_on_dataset (evaluation.py:2157-2305): the eval-mode forward
+    of every image, ONE statistics launch over all of them, and the reference's fold.
+
+    Each image is forwarded on its own, as the reference's forward_single_image_tensor does (net.py:265-299): with
+    normalize=True the network divides by a norm that only broadcasts per image for a batch of one (net.py:256-259), so
+    a batched forward would normalise the wrong images.  Everything runs on the device that holds dcn's parameters.
+
+    rgbs   [N,3,H,W] normalised image tensor, or a sequence of [3,H,W] ones (dataset.rgb_image_to_tensor's output)
+    masks  [N,H,W] (or a sequence of [H,W]) masks, 1 on the object; tensors or arrays
+    -> the reference's {'entire_image': {...}, 'mask_image': {...}} dict of lists (fold_descriptor_statistics)."""
+    imgs = rgbs if isinstance(rgbs, torch.Tensor) else torch.stack([torch.as_tensor(x) for x in rgbs])
+    if isinstance(masks, torch.Tensor):
+        mk = masks
+    else:
+        mk = torch.stack([m if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m)) for m in masks])
+    n = imgs.shape[0]
+    if imgs.dim() != 4 or imgs.shape[1] != 3 or mk.dim() != 3 or mk.shape[0] != n:
+        raise ValueError("rgbs must be [N,3,H,W] and masks [N,H,W] (got %s and %s)" % (tuple(imgs.shape), tuple(mk.shape)))
+    if mk.dtype not in (torch.float32, torch.uint8, torch.bool):
+        mk = mk.to(torch.float32)
+    dev = next(dcn.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("dcn must be on a CUDA device: this path has no CPU fallback")
+    dcn.eval()
+    H, W = imgs.shape[2], imgs.shape[3]
+    with torch.cuda.device(dev), torch.no_grad():
+        res = torch.empty(n, dcn.descriptor_dimension, H, W, dtype=torch.float32, device=dev)
+        for i in range(n):
+            x = imgs[i:i + 1].detach().to(device=dev, dtype=torch.float32).contiguous()
+            res[i:i + 1] = dcn.forward(x)
+        per_image = descriptor_statistics(res.permute(0, 2, 3, 1), mk.to(dev))
+    return fold_descriptor_statistics(per_image, n)
+
+
+def save_descriptor_statistics(stats, filename):
+    """utils.saveToYaml (dense_correspondence_manipulation/utils/utils.py:29-44), as compute_descriptor_statistics_on_dataset
+    writes descriptor_statistics.yaml into the network's parameter folder."""
+    import yaml
+    with open(filename, 'w') as outfile:
+        yaml.dump(stats, outfile, default_flow_style=False)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Across-object analysis (evaluate_network_across_objects, evaluation.py:305-338, 784-858, 977-1004)
+
+class DCNEvaluationPandaTemplateAcrossObject(PandaDataFrameWrapper):
+    """evaluation.py:66-76."""
+    columns = ['scene_name_a', 'scene_name_b', 'img_a_idx', 'img_b_idx', 'object_id_a', 'object_id_b',
+               'norm_diff_descriptor_best_match']
+
+    def __init__(self):
+        PandaDataFrameWrapper.__init__(self, DCNEvaluationPandaTemplateAcrossObject.columns)
+
+
+def best_match_batch(res_a, res_b, uv_a, pair):
+    """find_best_match (net.py:488-525) for Q query pixels over N image pairs in one launch (csrc/match_stats.cu).
+
+    res_a, res_b  [N,H,W,D] (or [H,W,D]) float32 CUDA, any strides; uv_a [Q,2] int64 CUDA (u, v) pixels of image A;
+    pair [Q] int64 CUDA, the image pair of each query (keeping one pair's queries together is fastest).
+    -> (best_uv [Q,2] int64, best_diff [Q] float32, bad_queries [1] int64) CUDA tensors, no host synchronisation.
+    best_diff is find_best_match's best_match_diff bit for bit (numpy's float32 arithmetic on a contiguous array); ties go
+    to the first pixel in row-major order.  Queries out of range get (-1, -1), NaN and are counted in bad_queries."""
+    if not isinstance(res_a, torch.Tensor) or not isinstance(res_b, torch.Tensor):
+        raise RuntimeError("res_a and res_b must be CUDA tensors")
+    N.require_cuda_f32(res_a, "res_a", contiguous=False); N.require_cuda_f32(res_b, "res_b", contiguous=False)
+    res_a = _batched(res_a, "res_a", 4); res_b = _batched(res_b, "res_b", 4, device=res_a.device)
+    dev = res_a.device
+    n, H, W, D = res_b.shape
+    if tuple(res_a.shape) != (n, H, W, D):
+        raise RuntimeError("res_a %s and res_b %s must have the same shape" % (tuple(res_a.shape), tuple(res_b.shape)))
+    if not 1 <= D <= MAX_D:
+        raise RuntimeError("descriptor dimension %d outside 1..%d" % (D, MAX_D))
+    uv_a = _index(uv_a, "uv_a", (2,), dev); pair = _index(pair, "pair", (), dev)
+    Q = uv_a.shape[0]
+    if pair.shape[0] != Q:
+        raise RuntimeError("uv_a and pair must have the same length")
+    uv = torch.empty(Q, 2, dtype=torch.int64, device=dev)
+    diff = torch.empty(Q, dtype=torch.float32, device=dev)
+    bad = torch.empty(1, dtype=torch.int64, device=dev)
+    nb = N.lib.ddn_best_match_batch_scratch_bytes(Q)
+    if nb == 0:
+        raise N.DdnError(N.lib.ddn_last_error().decode())
+    scratch = torch.empty(nb, dtype=torch.uint8, device=dev)
+    hp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    sa = np.array(res_a.stride(), dtype=np.int64); sb = np.array(res_b.stride(), dtype=np.int64)
+    N.check(N.lib.ddn_best_match_batch(N.ptr(res_a), hp(sa), N.ptr(res_b), hp(sb), n, H, W, D, N.ptr(pair), N.ptr(uv_a), Q,
+                                       N.ptr(uv), N.ptr(diff), N.ptr(bad), N.ptr(scratch), nb, N.stream_ptr()))
+    return uv, diff, bad
+
+
+def across_object_analysis(res_a, res_b, mask_a, pair=None, num_uv_a_samples=100, generator=None):
+    """single_across_object_image_pair_quantitative_analysis (evaluation.py:784-858) for a batch of N image pairs, from
+    descriptor images the device already holds: ``num_uv_a_samples`` pixels are drawn from each mask_a on the device (the
+    route quantitative_analysis_on_pair takes) and every one's best match in res_b is found in ONE launch.
+
+    res_a, res_b  [N,H,W,D] (or [H,W,D]) float32 CUDA descriptor images of object A and object B, any strides
+    mask_a        [N,H,W] (or [H,W]) masks of object A, 1 on the object
+    pair          None, or N dicts holding the template's other columns (scene_name_a, scene_name_b, img_a_idx,
+                  img_b_idx, object_id_a, object_id_b); a missing key leaves its column NaN
+    generator     a CUDA torch.Generator or None
+    -> dict of host numpy arrays, one row per sample: the columns of DCNEvaluationPandaTemplateAcrossObject,
+    "uv_a" / "uv_b" [R,2] (u, v) and "pair" [R].  A pair with an empty mask_a gives no rows (the reference returns an empty
+    list).  The reference draws with random.sample (without replacement, and it raises when the mask has fewer than
+    num_uv_a_samples pixels); this draws uniformly with replacement, so the sampled pixels differ, each row's value for
+    its uv_a does not."""
+    from . import sampling
+    if not isinstance(res_a, torch.Tensor) or not res_a.is_cuda:
+        raise RuntimeError("res_a must be a CUDA tensor: this path has no CPU fallback")
+    ra = _batched(res_a, "res_a", 4)
+    n, H, W, _ = ra.shape
+    dev = ra.device
+    ma = mask_a if isinstance(mask_a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(mask_a))
+    ma = _batched(ma.to(dev), "mask_a", 3).to(torch.float32).contiguous()
+    if tuple(ma.shape) != (n, H, W):
+        raise RuntimeError("mask_a must have shape %s (got %s)" % ((n, H, W), tuple(ma.shape)))
+    if pair is not None and len(pair) != n:
+        raise ValueError("pair must hold one dict per image pair (%d, got %d)" % (n, len(pair)))
+    k = int(num_uv_a_samples)
+    counts = torch.count_nonzero(ma.view(n, -1), dim=1).cpu().numpy()
+    keep = [i for i in range(n) if counts[i] > 0]
+    cols = {c: np.array([], dtype=object if c != 'norm_diff_descriptor_best_match' else np.float32)
+            for c in DCNEvaluationPandaTemplateAcrossObject.columns}
+    if not keep or k <= 0:
+        cols.update(uv_a=np.zeros((0, 2), np.int64), uv_b=np.zeros((0, 2), np.int64), pair=np.zeros(0, np.int64))
+        return cols
+    dummy = torch.zeros(1, dtype=torch.int64, device=dev)
+    flat = torch.cat([sampling.sample_non_matches(dummy, ma[i], (H, W), k, generator=generator)[1] for i in keep])
+    pidx = torch.tensor(keep, dtype=torch.int64, device=dev).repeat_interleave(k)
+    uv_a = torch.stack([flat % W, flat // W], 1)
+    uv_b, diff, _ = best_match_batch(ra, res_b, uv_a, pidx)
+    rows = pidx.cpu().numpy()
+    out = {'norm_diff_descriptor_best_match': diff.cpu().numpy(), 'uv_a': uv_a.cpu().numpy(), 'uv_b': uv_b.cpu().numpy(),
+           'pair': rows}
+    for c in DCNEvaluationPandaTemplateAcrossObject.columns[:-1]:
+        out[c] = np.array([(pair[i].get(c, np.nan) if pair is not None else np.nan) for i in rows], dtype=object)
+    return out
