@@ -154,6 +154,26 @@ int ddn_net_backward(int arch, const float* dy, const float* dlow_nhwc, const fl
                      ddn_grad_bucket_fn on_bucket, void* user, void* stream);
 /* 4 buckets for both architectures: layer4 + fc, layer3, layer2, layer1 + stem. */
 int ddn_net_grad_buckets(int arch, int D, int64_t* offsets, int cap);
+
+/* The three calls above with a `flags` argument (0 = exactly the calls above).
+ *   DDN_NET_UNIT_DESCRIPTORS: y is written with unit-length descriptors, y[:, p] = x / ||x|| for the bilinear upsample x of
+ *   every pixel p -- the reference's `normalize` option (dense_correspondence/network/dense_correspondence_network.py:256-259)
+ *   applied to each image on its own.  low_nhwc_out stays the un-normalised map.  The backward then takes dy through the
+ *   normalisation's Jacobian (dy - y (y.dy)) / ||x|| before the upsample's adjoint; dlow_nhwc is added as it is (the loss
+ *   kernels with DDN_LOWRES_UNIT already applied the Jacobian).  No epsilon: a pixel whose upsampled descriptor is zero gets
+ *   NaN, as x / ||x|| does in fp32.  Forward and backward of one step take the same flags, and the workspace is sized by
+ *   ddn_net_workspace_bytes_v2 with them (a backward with the flag needs B*D*H*W more floats). */
+enum { DDN_NET_UNIT_DESCRIPTORS = 1 };
+size_t ddn_net_workspace_bytes_v2(int arch, int B, int H, int W, int D, int mode, int precision, int flags);
+int ddn_net_forward_v2(int arch, const float* x, const float* params, float* buffers, float* y,
+                       void* workspace, size_t workspace_bytes,
+                       int B, int H, int W, int D,
+                       int mode, int bn_groups, float momentum, float eps, int precision,
+                       float* low_nhwc_out, int flags, void* stream);
+int ddn_net_backward_v2(int arch, const float* dy, const float* dlow_nhwc, const float* params, float* grads,
+                        void* workspace, size_t workspace_bytes,
+                        int B, int H, int W, int D, int mode, int bn_groups, float eps, int precision, int flags,
+                        ddn_grad_bucket_fn on_bucket, void* user, void* stream);
 size_t ddn_net_weight_cache_bytes(int arch, int D);
 
 /* ------------------------------------------------------------------------------------------
@@ -225,6 +245,19 @@ int ddn_contrastive_terms_backward_lowres(const float* low_a, const float* low_b
                                           const ddn_loss_term* terms_host, int n_terms,
                                           const float* coef, const float* upstream,
                                           float* dlow_a, float* dlow_b, double* scratch, void* stream);
+
+/* The same two with a `flags` argument (0 = exactly the calls above).
+ *   DDN_LOWRES_UNIT: every sampled descriptor is the blend x normalised to unit length, y = x / ||x|| (the images are the
+ *   DDN_NET_UNIT_DESCRIPTORS output of the network), in every term kind; the backward applies (g - y (y.g)) / ||x|| to each
+ *   side's gradient before the scatter.  A zero blend gives NaN descriptors (no epsilon). */
+enum { DDN_LOWRES_UNIT = 1 };
+int ddn_contrastive_terms_forward_lowres_v2(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
+                                            const ddn_loss_term* terms_host, int n_terms,
+                                            double* sums, int64_t* counts, int flags, void* stream);
+int ddn_contrastive_terms_backward_lowres_v2(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
+                                             const ddn_loss_term* terms_host, int n_terms,
+                                             const float* coef, const float* upstream,
+                                             float* dlow_a, float* dlow_b, double* scratch, int flags, void* stream);
 
 /* loss_composer.get_within_scene_loss (dense_correspondence/loss_functions/loss_composer.py:70-143)
  * evaluated on the device from the sums/counts of terms ordered {match, masked, background[, blind]}:
@@ -354,6 +387,12 @@ int ddn_conv2d_backward_data_bn_stats(const float* w_oihw, const float* dy_nhwc,
  * (nn.functional.upsample_bilinear, resnet_dilated.py:320) and its adjoint. */
 int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, int h, int w, int H, int W, void* stream);
 int ddn_upsample_bilinear_backward(const float* dy, float* dx, int NC, int h, int w, int H, int W, void* stream);
+/* The same resize of N images of D maps [N, D, h, w] -> [N, D, H, W] with every output pixel's D-vector normalised to unit
+ * length (y = x / ||x||, the network's DDN_NET_UNIT_DESCRIPTORS output; 1 <= D <= 32; a zero vector gives NaN), and its
+ * adjoint: dx [N, D, h, w] = upsample^T((dy - y (y.dy)) / ||x||), with `scratch` N*D*H*W floats for the middle term. */
+int ddn_upsample_bilinear_unit_forward(const float* x, float* y, int N, int D, int h, int w, int H, int W, void* stream);
+int ddn_upsample_bilinear_unit_backward(const float* x, const float* dy, float* dx, float* scratch, int N, int D, int h, int w,
+                                        int H, int W, void* stream);
 
 /* The scoring layer fc = nn.Conv2d(C, D, 1) with bias (resnet_dilated.py:298 for C = 512, :414 for C = 2048) on the trunk's
  * channels-last features, and its backward.  feat [N*Mimg, C] fp32, or its bf16 operand planes (feat = hi + lo; feat_lo may be

@@ -16,6 +16,8 @@ ARCH_RESNET34_8S, ARCH_RESNET50_8S = 0, 1
 GRAD_BUCKET_FN = ctypes.CFUNCTYPE(None, ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int64)
 TERM_MATCH, TERM_HINGE, TERM_HINGE_INV = 0, 1, 2
 TERM_PIXEL_WEIGHT = 1
+NET_UNIT_DESCRIPTORS = 1     # ddn_net_*_v2 flags: unit-length descriptors (the reference's `normalize`, per pixel)
+LOWRES_UNIT = 1              # ddn_contrastive_terms_*_lowres_v2 flags: the sampled descriptors are normalised to unit length
 MAX_TERMS = 8
 
 c_f32p = ctypes.POINTER(ctypes.c_float)
@@ -122,6 +124,10 @@ _SIGNATURES = {
     "ddn_contrastive_terms_forward_lowres": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp, vp]),
     "ddn_contrastive_terms_backward_lowres": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32,
                                                     vp, vp, vp, vp, vp, vp]),
+    "ddn_contrastive_terms_forward_lowres_v2": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp,
+                                                      i32, vp]),
+    "ddn_contrastive_terms_backward_lowres_v2": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(LossTerm), i32,
+                                                       vp, vp, vp, vp, vp, i32, vp]),
     "ddn_resnet34_8s_grad_buckets": (i32, [i32, ctypes.POINTER(i64), i32]),
     "ddn_net_param_table": (i32, [i32, i32, ctypes.POINTER(TensorEntry), i32]),
     "ddn_net_buffer_table": (i32, [i32, ctypes.POINTER(TensorEntry), i32]),
@@ -132,6 +138,9 @@ _SIGNATURES = {
     "ddn_net_forward": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, f32, i32, vp, vp]),
     "ddn_net_backward": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, i32, GRAD_BUCKET_FN, vp, vp]),
     "ddn_net_grad_buckets": (i32, [i32, i32, ctypes.POINTER(i64), i32]),
+    "ddn_net_workspace_bytes_v2": (sz, [i32] * 8),
+    "ddn_net_forward_v2": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, f32, i32, vp, i32, vp]),
+    "ddn_net_backward_v2": (i32, [i32, vp, vp, vp, vp, vp, sz, i32, i32, i32, i32, i32, i32, f32, i32, i32, GRAD_BUCKET_FN, vp, vp]),
     "ddn_contrastive_terms_forward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32, vp, vp, vp]),
     "ddn_contrastive_terms_backward": (i32, [vp, vp, i64, i64, i64, i32, i64, i32, i32, ctypes.POINTER(LossTerm), i32,
                                              vp, vp, vp, vp, vp]),
@@ -151,6 +160,8 @@ _SIGNATURES = {
     "ddn_batchnorm_backward": (i32, [vp] * 10 + [i64, i32, i32, vp, sz, vp]),
     "ddn_upsample_bilinear_forward": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
     "ddn_upsample_bilinear_backward": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+    "ddn_upsample_bilinear_unit_forward": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    "ddn_upsample_bilinear_unit_backward": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "ddn_fc_workspace_bytes": (sz, [i32, i32]),
     "ddn_fc_forward": (i32, [vp] * 7 + [i64, i32, i32, i32, vp]),
     "ddn_fc_backward": (i32, [vp] * 8 + [i64, i32, i32, i32, vp, sz, vp]),

@@ -169,8 +169,9 @@ def _gather_compose(ctx, pred_a, pred_b, image_width, terms, cfg, compose):
     return _fused_outputs(ctx, counts, five)
 
 
-def _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, compose):
-    """Forward of the fused losses through the bilinear upsample: one gather launch, one ``compose`` launch."""
+def _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, compose, unit):
+    """Forward of the fused losses through the bilinear upsample: one gather launch, one ``compose`` launch.  ``unit``: the
+    blended descriptors are normalised to unit length first (DDN_LOWRES_UNIT)."""
     B, _, D = low_a.shape
     h, w, H, W = geom
     T = len(terms)
@@ -181,11 +182,12 @@ def _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, compose):
     five = torch.empty(5, dtype=torch.float32, device=dev)
     coef = torch.empty(B, T, dtype=torch.float32, device=dev)
     st = N.stream_ptr()
-    N.check(N.lib.ddn_contrastive_terms_forward_lowres(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, arr, T,
-                                                       N.ptr(sums), N.ptr(counts), st))
+    flags = N.LOWRES_UNIT if unit else 0
+    N.check(N.lib.ddn_contrastive_terms_forward_lowres_v2(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, arr, T,
+                                                          N.ptr(sums), N.ptr(counts), flags, st))
     compose(sums, counts, cfg, five, coef, st)
     ctx.save_for_backward(low_a, low_b, coef)
-    ctx.arr, ctx.keep, ctx.geom = arr, keep, geom
+    ctx.arr, ctx.keep, ctx.geom, ctx.flags = arr, keep, geom, flags
     return _fused_outputs(ctx, counts, five)
 
 
@@ -220,11 +222,12 @@ class _PairTypes(_WithinScene):
 class _WithinSceneLowres(torch.autograd.Function):
     """within_scene_loss fused with the bilinear upsample: the descriptors are blended from the low-resolution maps
     ``low_a`` / ``low_b`` [B, h*w, D] (csrc/loss_lowres.cu); the gradient is scattered into d(low) -- the full-resolution
-    descriptor images and their gradients are never read or written."""
+    descriptor images and their gradients are never read or written.  ``unit``: every blended descriptor is normalised to
+    unit length (the images are unit-descriptor outputs of the network)."""
 
     @staticmethod
-    def forward(ctx, low_a, low_b, geom, terms, cfg):
-        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _within_scene_compose)
+    def forward(ctx, low_a, low_b, geom, terms, cfg, unit=False):
+        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _within_scene_compose, unit)
 
     @staticmethod
     def backward(ctx, dloss, _drest, _dcounts):
@@ -235,18 +238,24 @@ class _WithinSceneLowres(torch.autograd.Function):
         db = torch.zeros_like(low_b)
         up = dloss.to(torch.float32).contiguous()
         scratch = torch.empty(2 * low_a.numel(), dtype=torch.float64, device=low_a.device)    # the fp64 scatter accumulator
-        N.check(N.lib.ddn_contrastive_terms_backward_lowres(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, ctx.arr, len(ctx.arr),
-                                                            N.ptr(coef), N.ptr(up), N.ptr(da), N.ptr(db), N.ptr(scratch),
-                                                            N.stream_ptr()))
-        return da, db, None, None, None
+        N.check(N.lib.ddn_contrastive_terms_backward_lowres_v2(N.ptr(low_a), N.ptr(low_b), B, h, w, H, W, D, ctx.arr,
+                                                               len(ctx.arr), N.ptr(coef), N.ptr(up), N.ptr(da), N.ptr(db),
+                                                               N.ptr(scratch), ctx.flags, N.stream_ptr()))
+        return da, db, None, None, None, None
 
 
 class _PairTypesLowres(_WithinSceneLowres):
     """``_PairTypes`` through the bilinear upsample (the gather and scatter of ``_WithinSceneLowres``)."""
 
     @staticmethod
-    def forward(ctx, low_a, low_b, geom, terms, cfg):
-        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _pair_type_compose)
+    def forward(ctx, low_a, low_b, geom, terms, cfg, unit=False):
+        return _gather_compose_lowres(ctx, low_a, low_b, geom, terms, cfg, _pair_type_compose, unit)
+
+
+def _unpack_lowres(lowres):
+    """(low_a, low_b, geom) or (low_a, low_b, geom, unit) -> (low_a, low_b, geom, unit)"""
+    low_a, low_b, geom = lowres[:3]
+    return low_a, low_b, geom, bool(lowres[3]) if len(lowres) > 3 else False
 
 
 def within_scene_loss(pred_a, pred_b, image_width, terms, match_loss_weight, non_match_loss_weight,
@@ -268,9 +277,9 @@ def within_scene_loss(pred_a, pred_b, image_width, terms, match_loss_weight, non
                 keep.append(t)
                 setattr(cfg, field, t.data_ptr())
     cfg._keep = keep
-    if lowres is not None:        # (low_a, low_b, (h, w, H, W)): both images are bilinear upsamples of these maps
-        low_a, low_b, geom = lowres
-        return _WithinSceneLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg)
+    if lowres is not None:        # (low_a, low_b, (h, w, H, W)[, unit]): both images are bilinear upsamples of these maps
+        low_a, low_b, geom, unit = _unpack_lowres(lowres)
+        return _WithinSceneLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg, unit)
     return _WithinScene.apply(pred_a, pred_b, int(image_width), list(terms), cfg)
 
 
@@ -300,6 +309,6 @@ def pair_type_loss(pred_a, pred_b, image_width, terms, pair_type, match_loss_wei
         setattr(cfg, field, t.data_ptr())
     cfg._keep, cfg._pair_type = keep, pair_type.contiguous()
     if lowres is not None:
-        low_a, low_b, geom = lowres
-        return _PairTypesLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg)
+        low_a, low_b, geom, unit = _unpack_lowres(lowres)
+        return _PairTypesLowres.apply(low_a.contiguous(), low_b.contiguous(), geom, list(terms), cfg, unit)
     return _PairTypes.apply(pred_a, pred_b, int(image_width), list(terms), cfg)

@@ -85,6 +85,8 @@ int launch_fc_backward(const float* dlow, const float* feat, const __nv_bfloat16
                        float* dfeat, float* dw, float* dbias, float* part, int64_t Mimg, int N, int C, int D, cudaStream_t st);
 int launch_upsample_fwd(const float* x, float* y, int NC, int h, int w, int H, int W, cudaStream_t st);
 int launch_upsample_bwd(const float* dy, float* dx, int NC, int h, int w, int H, int W, cudaStream_t st);
+int launch_upsample_unit_fwd(const float* x, float* y, int N, int D, int h, int w, int H, int W, cudaStream_t st);
+int launch_upsample_unit_bwd(const float* x, const float* dy, float* dx, float* g, int N, int D, int h, int w, int H, int W, cudaStream_t st);
 int launch_fill_zero(void* p, size_t bytes, cudaStream_t st);
 
 }  // namespace ddn

@@ -218,12 +218,15 @@ struct Plan {
   size_t acc, sums;                   // BatchNorm accumulator (bn_stats.cuh) and the backward's per-group sums
   size_t dwp_all;                     // [n_params + 64*192] doubles: every conv's [taps][Cout][Cin] gradient accumulator (tensor-core modes)
   size_t scratch_elems;
+  size_t unit_dy;                     // DDN_NET_UNIT_DESCRIPTORS with a backward: [B, D, H, W] cotangent through the normalisation
+  int flags;
   size_t total;
 };
 
 static float* stat_mean(char* ws, const ConvBufs& cb) { return reinterpret_cast<float*>(ws + cb.stats); }
 
-static int make_plan(Plan* p, int arch, int B, int H, int W, int D, int mode, int precision) {
+static int make_plan(Plan* p, int arch, int B, int H, int W, int D, int mode, int precision, int flags = 0) {
+  DDN_CHECK_ARG((flags & ~DDN_NET_UNIT_DESCRIPTORS) == 0, "unknown network flags 0x%x", flags);
   DDN_CHECK_ARG(arch_ok(arch), "unknown architecture id %d", arch);
   DDN_CHECK_ARG(B >= 1 && H >= 32 && W >= 32 && H % 8 == 0 && W % 8 == 0, "need B>=1 and H, W multiples of 8 (>=32); got B=%d H=%d W=%d", B, H, W);
   DDN_CHECK_ARG(D >= 1 && D <= 32, "descriptor dimension must be in [1,32] (got %d)", D);
@@ -314,6 +317,9 @@ static int make_plan(Plan* p, int arch, int B, int H, int W, int D, int mode, in
   p->wws = alloc(p->tc ? tc_weight_ws_bytes() : 0);
   p->dwp_all = (p->tc && mode != DDN_MODE_INFER) ? alloc(sizeof(double) * (size_t)(s.n_params + 64 * 192)) : 0;
   p->fc_part = mode != DDN_MODE_INFER ? f32((int64_t)fc_part_floats(s.fc_cin, D)) : 0;
+  // last, so that a plan without the flag is byte for byte the plan of ddn_net_workspace_bytes
+  p->flags = flags;
+  p->unit_dy = ((flags & DDN_NET_UNIT_DESCRIPTORS) && mode != DDN_MODE_INFER) ? f32((int64_t)B * D * H * W) : 0;
   p->total = cur;
   return 0;
 }
@@ -548,7 +554,10 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   DDN_TRY(launch_fc_forward(feat_planes ? nullptr : cur, feat_planes ? c.h(cur_p.hi) : nullptr,
                             (feat_planes && want_lo) ? c.h(cur_p.lo) : nullptr, c.params + s.fc_w, c.params + s.fc_b, c.f(p.low),
                             low_nhwc, (int64_t)h8 * w8, B, s.fc_cin, p.D, c.st));
-  DDN_TRY(launch_upsample_fwd(c.f(p.low), y, B * p.D, h8, w8, p.H, p.W, c.st));
+  if (p.flags & DDN_NET_UNIT_DESCRIPTORS)    // y = x / ||x|| per pixel (dense_correspondence_network.py:256-259)
+    DDN_TRY(launch_upsample_unit_fwd(c.f(p.low), y, B, p.D, h8, w8, p.H, p.W, c.st));
+  else
+    DDN_TRY(launch_upsample_fwd(c.f(p.low), y, B * p.D, h8, w8, p.H, p.W, c.st));
   return 0;
 }
 
@@ -644,7 +653,11 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
   if (p.tc) DDN_CUDA(cudaMemsetAsync(c.d(p.dwp_all), 0, sizeof(double) * (size_t)(s.n_params + 64 * 192), c.st));
   const BlockBufs& last = p.blk.back();
   // d(low) = upsample^T(dy) [+ the gradient the fused loss scattered straight into the low-resolution map]
-  if (dy) DDN_TRY(launch_upsample_bwd(dy, c.f(p.dlow), B * p.D, h8, w8, p.H, p.W, c.st));
+  // (unit descriptors: dy first goes through the normalisation's Jacobian; dlow_nhwc already has, in the fused loss)
+  if (dy && (p.flags & DDN_NET_UNIT_DESCRIPTORS))
+    DDN_TRY(launch_upsample_unit_bwd(c.f(p.low), dy, c.f(p.dlow), c.f(p.unit_dy), B, p.D, h8, w8, p.H, p.W, c.st));
+  else if (dy)
+    DDN_TRY(launch_upsample_bwd(dy, c.f(p.dlow), B * p.D, h8, w8, p.H, p.W, c.st));
   if (dlow_nhwc) DDN_TRY(launch_add_lowres_nhwc(dlow_nhwc, c.f(p.dlow), (int64_t)h8 * w8, B, p.D, dy ? 1 : 0, c.st));
   int cur = 0;   // index of the scratch buffer holding d(block output)
   DDN_TRY(launch_fc_backward(c.f(p.dlow), p.tc ? nullptr : c.f(last.out), p.tc ? c.h(last.out_p.hi) : nullptr,
@@ -811,8 +824,11 @@ extern "C" size_t ddn_net_weight_cache_bytes(int arch, int D) {
   return (size_t)get_spec(arch, D).n_params * 2 * 2 * sizeof(__nv_bfloat16) + 4096;
 }
 extern "C" size_t ddn_net_workspace_bytes(int arch, int B, int H, int W, int D, int mode, int precision) {
+  return ddn_net_workspace_bytes_v2(arch, B, H, W, D, mode, precision, 0);
+}
+extern "C" size_t ddn_net_workspace_bytes_v2(int arch, int B, int H, int W, int D, int mode, int precision, int flags) {
   Plan p;
-  if (make_plan(&p, arch, B, H, W, D, mode, precision) != 0) return 0;
+  if (make_plan(&p, arch, B, H, W, D, mode, precision, flags) != 0) return 0;
   return p.total;
 }
 
@@ -830,10 +846,17 @@ extern "C" int ddn_net_forward(int arch, const float* x, const float* params, fl
                                void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
                                int mode, int bn_groups, float momentum, float eps, int precision, float* low_nhwc_out,
                                void* stream) {
+  return ddn_net_forward_v2(arch, x, params, buffers, y, workspace, workspace_bytes, B, H, W, D, mode, bn_groups, momentum, eps, precision,
+                            low_nhwc_out, 0, stream);
+}
+extern "C" int ddn_net_forward_v2(int arch, const float* x, const float* params, float* buffers, float* y,
+                                  void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                                  int mode, int bn_groups, float momentum, float eps, int precision, float* low_nhwc_out,
+                                  int flags, void* stream) {
   DDN_CHECK_ARG(x && params && buffers && y, "null tensor");
   DDN_TRY(check_groups(B, bn_groups));
   Plan p;
-  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision));
+  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision, flags));
   DDN_TRY(check_ws(p, workspace, workspace_bytes));
   Ctx c = {&get_spec(arch, D), &p, (char*)workspace, params, buffers, nullptr, (cudaStream_t)stream, momentum, eps, mode, bn_groups};
   return net_forward(c, x, y, low_nhwc_out);
@@ -843,11 +866,18 @@ extern "C" int ddn_net_backward(int arch, const float* dy, const float* dlow_nhw
                                 void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
                                 int mode, int bn_groups, float eps, int precision,
                                 ddn_grad_bucket_fn on_bucket, void* user, void* stream) {
+  return ddn_net_backward_v2(arch, dy, dlow_nhwc, params, grads, workspace, workspace_bytes, B, H, W, D, mode, bn_groups, eps, precision,
+                             0, on_bucket, user, stream);
+}
+extern "C" int ddn_net_backward_v2(int arch, const float* dy, const float* dlow_nhwc, const float* params, float* grads,
+                                   void* workspace, size_t workspace_bytes, int B, int H, int W, int D,
+                                   int mode, int bn_groups, float eps, int precision, int flags,
+                                   ddn_grad_bucket_fn on_bucket, void* user, void* stream) {
   DDN_CHECK_ARG((dy || dlow_nhwc) && params && grads, "null tensor");
   DDN_CHECK_ARG(mode == DDN_MODE_TRAIN || mode == DDN_MODE_EVAL_SAVE, "backward needs a forward that kept its activations (mode %d)", mode);
   DDN_TRY(check_groups(B, bn_groups));
   Plan p;
-  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision));
+  DDN_TRY(make_plan(&p, arch, B, H, W, D, mode, precision, flags));
   DDN_TRY(check_ws(p, workspace, workspace_bytes));
   Ctx c = {&get_spec(arch, D), &p, (char*)workspace, params, nullptr, grads, (cudaStream_t)stream, 0.f, eps, mode, bn_groups};
   return net_backward(c, dy, dlow_nhwc, on_bucket, user);

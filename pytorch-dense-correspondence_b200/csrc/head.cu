@@ -328,6 +328,76 @@ upsample_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int NC
   }
 }
 
+// ---- unit-length descriptors (the reference's `normalize` option, dense_correspondence_network.py:256-259, per pixel): the
+// bilinear blend x of all D maps of one output pixel, then y = x / ||x||.  One thread per output pixel; consecutive threads are
+// consecutive columns, so every channel's loads and stores are coalesced.  The blend is upsample_fwd_kernel's arithmetic.  A
+// zero blend gives NaN, as x / ||x|| does in fp32 (no epsilon).
+template <int DM>
+__device__ __forceinline__ float unit_blend(const float* __restrict__ x, int64_t n, int D, int h, int w, int oh, int ow, float sh, float sw,
+                                            float (&v)[DM]) {
+  int h0, h1, w0, w1; float lh, lw;
+  src_index(sh, oh, h, h0, h1, lh);
+  src_index(sw, ow, w, w0, w1, lw);
+  float s = 0.f;
+#pragma unroll
+  for (int c = 0; c < DM; ++c) {
+    v[c] = 0.f;
+    if (c < D) {
+      const float* m = x + (n * D + c) * h * w;
+      float top = (1.f - lw) * __ldg(m + h0 * w + w0) + lw * __ldg(m + h0 * w + w1);
+      float bot = (1.f - lw) * __ldg(m + h1 * w + w0) + lw * __ldg(m + h1 * w + w1);
+      v[c] = (1.f - lh) * top + lh * bot;
+      s = fmaf(v[c], v[c], s);
+    }
+  }
+  return sqrtf(s);
+}
+
+template <int DM>
+__global__ void __launch_bounds__(256)
+upsample_unit_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, int N, int D, int h, int w, int H, int W, float sh, float sw) {
+  pdl_prologue();
+  const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t n = i / HW, p = i - n * HW;
+    const int oh = (int)(p / W), ow = (int)(p - (int64_t)oh * W);
+    float v[DM];
+    const float nrm = unit_blend<DM>(x, n, D, h, w, oh, ow, sh, sw, v);
+#pragma unroll
+    for (int c = 0; c < DM; ++c)
+      if (c < D) y[(n * D + c) * HW + p] = v[c] / nrm;
+  }
+}
+
+// g = (dy - y (y.dy)) / ||x||: the full-resolution cotangent through the normalisation (x recomputed from the low-resolution
+// maps); upsample_bwd_kernel then takes g to the low-resolution maps
+template <int DM>
+__global__ void __launch_bounds__(256)
+unit_vjp_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ g, int N, int D, int h, int w, int H, int W,
+                float sh, float sw) {
+  pdl_prologue();
+  const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t n = i / HW, p = i - n * HW;
+    const int oh = (int)(p / W), ow = (int)(p - (int64_t)oh * W);
+    float v[DM], d[DM];
+    const float nrm = unit_blend<DM>(x, n, D, h, w, oh, ow, sh, sw, v);
+    float t = 0.f;
+#pragma unroll
+    for (int c = 0; c < DM; ++c) {
+      d[c] = 0.f;
+      if (c < D) {
+        d[c] = __ldg(dy + (n * D + c) * HW + p);
+        v[c] = v[c] / nrm;
+        t = fmaf(v[c], d[c], t);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < DM; ++c)
+      if (c < D) g[(n * D + c) * HW + p] = (d[c] - v[c] * t) / nrm;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 static int ew_blocks(int64_t total, int threads) { return (int)std::min<int64_t>(ceil_div(total, threads), (int64_t)num_sms() * 8); }
 
@@ -422,6 +492,27 @@ int launch_upsample_bwd(const float* dy, float* dx, int NC, int h, int w, int H,
   return 0;
 }
 
+int launch_upsample_unit_fwd(const float* x, float* y, int N, int D, int h, int w, int H, int W, cudaStream_t st) {
+  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD, "unit upsample: need 1 <= D <= %d (got %d)", FC_MAXD, D);
+  const int64_t total = (int64_t)N * H * W;
+  const float sh = ac_scale(h, H), sw = ac_scale(w, W);
+#define CALL(DM) DDN_LAUNCH(upsample_unit_fwd_kernel<DM>, ew_blocks(total, 256), 256, 0, st, x, y, N, D, h, w, H, W, sh, sw)
+  FC_DISPATCH(D, CALL);
+#undef CALL
+  return 0;
+}
+
+// g (N*D*H*W floats of scratch) = the cotangent through the normalisation, then dx = upsample^T(g)
+int launch_upsample_unit_bwd(const float* x, const float* dy, float* dx, float* g, int N, int D, int h, int w, int H, int W, cudaStream_t st) {
+  DDN_CHECK_ARG(D >= 1 && D <= FC_MAXD, "unit upsample: need 1 <= D <= %d (got %d)", FC_MAXD, D);
+  const int64_t total = (int64_t)N * H * W;
+  const float sh = ac_scale(h, H), sw = ac_scale(w, W);
+#define CALL(DM) DDN_LAUNCH(unit_vjp_kernel<DM>, ew_blocks(total, 256), 256, 0, st, x, dy, g, N, D, h, w, H, W, sh, sw)
+  FC_DISPATCH(D, CALL);
+#undef CALL
+  return launch_upsample_bwd(g, dx, N * D, h, w, H, W, st);
+}
+
 // dlow [N, D, Mimg] (+)= dlow_t [N, Mimg, D]: the gradient the fused loss scattered into the NHWC low-resolution map
 __global__ void add_lowres_nhwc_kernel(const float* __restrict__ dlow_t, float* __restrict__ dlow, int64_t Mimg, int N, int D, int accumulate) {
   pdl_prologue();
@@ -455,6 +546,23 @@ extern "C" int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, i
 extern "C" int ddn_upsample_bilinear_backward(const float* dy, float* dx, int NC, int h, int w, int H, int W, void* stream) {
   DDN_CHECK_ARG(dy && dx && NC > 0 && h > 0 && w > 0 && H > 0 && W > 0, "bad upsample arguments");
   return launch_upsample_bwd(dy, dx, NC, h, w, H, W, (cudaStream_t)stream);
+}
+
+static int check_unit_upsample(int N, int D, int h, int w, int H, int W) {
+  DDN_CHECK_ARG(N > 0 && D >= 1 && D <= FC_MAXD && h > 0 && w > 0 && H > 0 && W > 0 && (int64_t)N * D * H * W < (1LL << 40),
+                "bad unit upsample arguments (N=%d D=%d h=%d w=%d H=%d W=%d; 1 <= D <= %d)", N, D, h, w, H, W, FC_MAXD);
+  return 0;
+}
+extern "C" int ddn_upsample_bilinear_unit_forward(const float* x, float* y, int N, int D, int h, int w, int H, int W, void* stream) {
+  DDN_CHECK_ARG(x && y, "null tensor");
+  DDN_TRY(check_unit_upsample(N, D, h, w, H, W));
+  return launch_upsample_unit_fwd(x, y, N, D, h, w, H, W, (cudaStream_t)stream);
+}
+extern "C" int ddn_upsample_bilinear_unit_backward(const float* x, const float* dy, float* dx, float* scratch, int N, int D, int h, int w,
+                                                   int H, int W, void* stream) {
+  DDN_CHECK_ARG(x && dy && dx && scratch, "null tensor");
+  DDN_TRY(check_unit_upsample(N, D, h, w, H, W));
+  return launch_upsample_unit_bwd(x, dy, dx, scratch, N, D, h, w, H, W, (cudaStream_t)stream);
 }
 
 extern "C" size_t ddn_fc_workspace_bytes(int C, int D) { return fc_shape_ok(C, D) ? sizeof(float) * fc_part_floats(C, D) : 0; }

@@ -15,6 +15,11 @@
 // the channel-strided NCHW gather) to the 16 bytes of the two indices.
 //
 // Descriptor images: low_a / low_b [B, h*w, D] fp32 (what ddn_resnet34_8s_forward writes to `low_nhwc_out`).
+//
+// UNIT = true (DDN_LOWRES_UNIT): the descriptor is the blend x normalised to unit length, y = x / ||x||, which is what the
+// reference's `normalize` option computes per output pixel after its upsample (dense_correspondence_network.py:256-259).  The
+// forward scores y; the backward applies the normalisation's Jacobian dx = (g - y (y.g)) / ||x|| to each side's gradient g
+// before the scatter (||x|| recomputed from the 4 cells, nothing stored).  A zero blend gives NaN, as x / ||x|| does in fp32.
 #include "bn_stats.cuh"
 #include "loss.cuh"
 
@@ -85,7 +90,61 @@ __device__ __forceinline__ void descriptor_diff(const float* __restrict__ A, con
   }
 }
 
+// one side's blended descriptor x[0..D) of pixel `bl` (the arithmetic of descriptor_diff), channels >= D zero
 template <int D_T>
+__device__ __forceinline__ void descriptor_blend(const float* __restrict__ A, const Blend& bl, int D_rt, float (&x)[D_T > 0 ? D_T : LOSS_MAXD]) {
+  constexpr int DM = D_T > 0 ? D_T : LOSS_MAXD;
+  const int D = D_T > 0 ? D_T : D_rt;
+  const float* a00 = A + (size_t)bl.c00 * D; const float* a01 = A + (size_t)bl.c01 * D;
+  const float* a10 = A + (size_t)bl.c10 * D; const float* a11 = A + (size_t)bl.c11 * D;
+#pragma unroll
+  for (int c = 0; c < DM; ++c) {
+    x[c] = 0.f;
+    if (c < D) x[c] = blend1(__ldg(a00 + c), __ldg(a01 + c), __ldg(a10 + c), __ldg(a11 + c), bl.lh, bl.lw);
+  }
+}
+
+// x <- x / ||x|| over channels [0, D); returns ||x|| (0 gives NaN descriptors, as the division does)
+template <int DM>
+__device__ __forceinline__ float unit_normalize(float (&x)[DM], int D) {
+  float s = 0.f;
+#pragma unroll
+  for (int c = 0; c < DM; ++c) s = fmaf(x[c], x[c], s);
+  const float n = sqrtf(s);
+#pragma unroll
+  for (int c = 0; c < DM; ++c)
+    if (c < D) x[c] = x[c] / n;
+  return n;
+}
+
+// g <- (g - y (y.g)) / n: the vector-Jacobian product of y = x / ||x|| with n = ||x||
+template <int DM>
+__device__ __forceinline__ void unit_vjp(float (&g)[DM], const float (&y)[DM], float n, int D) {
+  float t = 0.f;
+#pragma unroll
+  for (int c = 0; c < DM; ++c)
+    if (c < D) t = fmaf(y[c], g[c], t);
+#pragma unroll
+  for (int c = 0; c < DM; ++c)
+    if (c < D) g[c] = (g[c] - y[c] * t) / n;
+}
+
+// unit descriptors of both sides and their difference d = ya - yb
+template <int D_T>
+__device__ __forceinline__ void descriptor_diff_unit(const float* __restrict__ A, const float* __restrict__ Bq, const Blend& ba, const Blend& bb,
+                                                     int D_rt, float (&d)[D_T > 0 ? D_T : LOSS_MAXD], float (&ya)[D_T > 0 ? D_T : LOSS_MAXD],
+                                                     float (&yb)[D_T > 0 ? D_T : LOSS_MAXD], float& na, float& nb) {
+  constexpr int DM = D_T > 0 ? D_T : LOSS_MAXD;
+  const int D = D_T > 0 ? D_T : D_rt;
+  descriptor_blend<D_T>(A, ba, D, ya);
+  descriptor_blend<D_T>(Bq, bb, D, yb);
+  na = unit_normalize<DM>(ya, D);
+  nb = unit_normalize<DM>(yb, D);
+#pragma unroll
+  for (int c = 0; c < DM; ++c) d[c] = ya[c] - yb[c];
+}
+
+template <int D_T, bool UNIT>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_fwd_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, int D_rt, float sh, float sw,
                        const __grid_constant__ DevTerms T, double* __restrict__ sums, unsigned long long* __restrict__ counts) {
@@ -108,7 +167,12 @@ loss_lowres_fwd_kernel(const float* __restrict__ la, const float* __restrict__ l
     if (na >= 0 && nb >= 0 && na < P && nb < P) {
       const Blend ba = blend_of(na, W, h, w, sh, sw), bb = blend_of(nb, W, h, w, sh, sw);
       float d[DM];
-      descriptor_diff<D_T>(A, Bq, ba, bb, D, d);
+      if constexpr (UNIT) {
+        float ya[DM], yb[DM], na, nb;
+        descriptor_diff_unit<D_T>(A, Bq, ba, bb, D, d, ya, yb, na, nb);
+      } else {
+        descriptor_diff<D_T>(A, Bq, ba, bb, D, d);
+      }
       float s2 = 0.f;
 #pragma unroll
       for (int c = 0; c < DM; ++c) s2 = fmaf(d[c], d[c], s2);
@@ -161,7 +225,7 @@ __device__ __forceinline__ void scatter_desc(double* __restrict__ dL, const Blen
   }
 }
 
-template <int D_T>
+template <int D_T, bool UNIT>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, int D_rt, float sh, float sw,
                        const __grid_constant__ DevTerms T, const float* __restrict__ coef, const float* __restrict__ upstream,
@@ -192,9 +256,11 @@ loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ l
 #pragma unroll
   for (int c = 0; c < DM; ++c) g[c] = 0.f;
   float scale = 0.f;
+  float ya[UNIT ? DM : 1], yb[UNIT ? DM : 1], nrm_a = 0.f, nrm_b = 0.f;    // UNIT: both sides' unit descriptors and norms
   if (ok) {
     ba = blend_of(na, W, h, w, sh, sw); bb = blend_of(nb, W, h, w, sh, sw);
-    descriptor_diff<D_T>(A, Bq, ba, bb, D, g);
+    if constexpr (UNIT) descriptor_diff_unit<D_T>(A, Bq, ba, bb, D, g, ya, yb, nrm_a, nrm_b);
+    else descriptor_diff<D_T>(A, Bq, ba, bb, D, g);
     float s2 = 0.f;
 #pragma unroll
     for (int c = 0; c < DM; ++c) s2 = fmaf(g[c], g[c], s2);
@@ -216,10 +282,14 @@ loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ l
     float gb[DM];
 #pragma unroll
     for (int c = 0; c < DM; ++c) gb[c] = -g[c];
+    if constexpr (UNIT) unit_vjp<DM>(gb, yb, nrm_b, D);
     scatter_desc<D_T>(dB, bb, D, gb);
   }
   if (!hinge) {
-    if (ok && scale != 0.f) scatter_desc<D_T>(dA, ba, D, g);
+    if (ok && scale != 0.f) {
+      if constexpr (UNIT) unit_vjp<DM>(g, ya, nrm_a, D);
+      scatter_desc<D_T>(dA, ba, D, g);
+    }
     return;
   }
   // runs of equal A indices (every match repeated k times consecutively, spartan_dataset_masked.py:853-854): one scatter per run
@@ -241,6 +311,7 @@ loss_lowres_bwd_kernel(const float* __restrict__ la, const float* __restrict__ l
     }
   }
   if (head && ok) {
+    if constexpr (UNIT) unit_vjp<DM>(g, ya, nrm_a, D);     // linear: the run's summed gradient takes the head's Jacobian once
     bool any = false;
 #pragma unroll
     for (int c = 0; c < DM; ++c) any = any || (g[c] != 0.f);
@@ -265,10 +336,35 @@ __device__ __forceinline__ float4 quad_diff(const float* __restrict__ A, const f
                      blend1(a00.w, a01.w, a10.w, a11.w, ba.lh, ba.lw) - blend1(b00.w, b01.w, b10.w, b11.w, bb.lh, bb.lw));
 }
 
+// one side's blended channel quad `sub` of pixel `bl` (the arithmetic of quad_diff)
+template <int LPP>
+__device__ __forceinline__ float4 quad_blend(const float* __restrict__ A, const Blend& bl, int sub) {
+  constexpr int D = 4 * LPP;
+  const float4 a00 = __ldg(reinterpret_cast<const float4*>(A + (size_t)bl.c00 * D) + sub), a01 = __ldg(reinterpret_cast<const float4*>(A + (size_t)bl.c01 * D) + sub);
+  const float4 a10 = __ldg(reinterpret_cast<const float4*>(A + (size_t)bl.c10 * D) + sub), a11 = __ldg(reinterpret_cast<const float4*>(A + (size_t)bl.c11 * D) + sub);
+  return make_float4(blend1(a00.x, a01.x, a10.x, a11.x, bl.lh, bl.lw), blend1(a00.y, a01.y, a10.y, a11.y, bl.lh, bl.lw),
+                     blend1(a00.z, a01.z, a10.z, a11.z, bl.lh, bl.lw), blend1(a00.w, a01.w, a10.w, a11.w, bl.lh, bl.lw));
+}
+__device__ __forceinline__ float dot4(float4 a, float4 b) { return fmaf(a.x, b.x, fmaf(a.y, b.y, fmaf(a.z, b.z, a.w * b.w))); }
+__device__ __forceinline__ float4 div4(float4 a, float n) { return make_float4(a.x / n, a.y / n, a.z / n, a.w / n); }
+// the sum of v over the LPP lanes of one index pair (every lane of the warp must call it)
+template <int LPP>
+__device__ __forceinline__ float pair_sum(float v) {
+#pragma unroll
+  for (int off = 1; off < LPP; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+// the quad layout of unit_vjp: g <- (g - y (y.g)) / n, y.g summed over the pair's lanes (every lane of the warp must call it)
+template <int LPP>
+__device__ __forceinline__ float4 quad_unit_vjp(float4 g, float4 y, float n) {
+  const float t = pair_sum<LPP>(dot4(y, g));
+  return make_float4((g.x - y.x * t) / n, (g.y - y.y * t) / n, (g.z - y.z * t) / n, (g.w - y.w * t) / n);
+}
+
 // LR_FWD_ITEMS index pairs per lane group in the forward: that many times fewer blocks = fewer contended atomics on the
 // B * n_terms accumulators (they bound the one-pair version), and 8 * LR_FWD_ITEMS loads in flight per lane
 constexpr int LR_FWD_ITEMS = 4;
-template <int LPP>
+template <int LPP, bool UNIT>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_fwd_quad_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, float sh, float sw,
                             const __grid_constant__ DevTerms T, double* __restrict__ sums, unsigned long long* __restrict__ counts) {
@@ -293,14 +389,37 @@ loss_lowres_fwd_quad_kernel(const float* __restrict__ la, const float* __restric
   }
   float s2[LR_FWD_ITEMS];
   bool ok[LR_FWD_ITEMS];
+  if constexpr (UNIT) {
+    float4 xa[LR_FWD_ITEMS], xb[LR_FWD_ITEMS];
 #pragma unroll
-  for (int k = 0; k < LR_FWD_ITEMS; ++k) {
-    ok[k] = na[k] >= 0 && nb[k] >= 0 && na[k] < P && nb[k] < P;
-    s2[k] = 0.f;
-    if (ok[k]) {
-      const Blend ba = blend_of(na[k], W, h, w, sh, sw), bb = blend_of(nb[k], W, h, w, sh, sw);
-      const float4 d = quad_diff<LPP>(A, Bq, ba, bb, sub);
-      s2[k] = fmaf(d.x, d.x, fmaf(d.y, d.y, fmaf(d.z, d.z, d.w * d.w)));
+    for (int k = 0; k < LR_FWD_ITEMS; ++k) {
+      ok[k] = na[k] >= 0 && nb[k] >= 0 && na[k] < P && nb[k] < P;
+      xa[k] = xb[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (ok[k]) {
+        xa[k] = quad_blend<LPP>(A, blend_of(na[k], W, h, w, sh, sw), sub);
+        xb[k] = quad_blend<LPP>(Bq, blend_of(nb[k], W, h, w, sh, sw), sub);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < LR_FWD_ITEMS; ++k) {
+      const float nrm_a = sqrtf(pair_sum<LPP>(dot4(xa[k], xa[k]))), nrm_b = sqrtf(pair_sum<LPP>(dot4(xb[k], xb[k])));
+      s2[k] = 0.f;
+      if (ok[k]) {
+        const float4 ya = div4(xa[k], nrm_a), yb = div4(xb[k], nrm_b);
+        const float4 d = make_float4(ya.x - yb.x, ya.y - yb.y, ya.z - yb.z, ya.w - yb.w);
+        s2[k] = dot4(d, d);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < LR_FWD_ITEMS; ++k) {
+      ok[k] = na[k] >= 0 && nb[k] >= 0 && na[k] < P && nb[k] < P;
+      s2[k] = 0.f;
+      if (ok[k]) {
+        const Blend ba = blend_of(na[k], W, h, w, sh, sw), bb = blend_of(nb[k], W, h, w, sh, sw);
+        const float4 d = quad_diff<LPP>(A, Bq, ba, bb, sub);
+        s2[k] = fmaf(d.x, d.x, fmaf(d.y, d.y, fmaf(d.z, d.z, d.w * d.w)));
+      }
     }
   }
   float acc = 0.f;
@@ -357,7 +476,7 @@ __device__ __forceinline__ void scatter_quad(double* __restrict__ dL, const Blen
   }
 }
 
-template <int LPP>
+template <int LPP, bool UNIT>
 __global__ void __launch_bounds__(LR_THREADS)
 loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restrict__ lb, int h, int w, int H, int W, float sh, float sw,
                             const __grid_constant__ DevTerms T, const float* __restrict__ coef, const float* __restrict__ upstream,
@@ -386,7 +505,20 @@ loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restric
   Blend ba = {}, bb = {};
   float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
   float s2 = 0.f;
-  if (ok) {
+  float4 ya = g, yb = g;                                 // UNIT: both sides' unit descriptors and norms
+  float nrm_a = 1.f, nrm_b = 1.f;
+  if constexpr (UNIT) {
+    if (ok) {
+      ba = blend_of(na, W, h, w, sh, sw); bb = blend_of(nb, W, h, w, sh, sw);
+      ya = quad_blend<LPP>(A, ba, sub); yb = quad_blend<LPP>(Bq, bb, sub);
+    }
+    nrm_a = sqrtf(pair_sum<LPP>(dot4(ya, ya))); nrm_b = sqrtf(pair_sum<LPP>(dot4(yb, yb)));
+    if (ok) {
+      ya = div4(ya, nrm_a); yb = div4(yb, nrm_b);
+      g = make_float4(ya.x - yb.x, ya.y - yb.y, ya.z - yb.z, ya.w - yb.w);
+      s2 = dot4(g, g);
+    }
+  } else if (ok) {
     ba = blend_of(na, W, h, w, sh, sw); bb = blend_of(nb, W, h, w, sh, sw);
     g = quad_diff<LPP>(A, Bq, ba, bb, sub);
     s2 = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, g.w * g.w)));
@@ -408,8 +540,11 @@ loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restric
     }
   }
   g.x *= scale; g.y *= scale; g.z *= scale; g.w *= scale;
-  if (ok && scale != 0.f) scatter_quad<LPP>(dB, bb, sub, make_float4(-g.x, -g.y, -g.z, -g.w));       // B side: random indices
+  float4 gb = make_float4(-g.x, -g.y, -g.z, -g.w);
+  if constexpr (UNIT) gb = quad_unit_vjp<LPP>(gb, yb, nrm_b);
+  if (ok && scale != 0.f) scatter_quad<LPP>(dB, bb, sub, gb);       // B side: random indices
   if (!hinge) {
+    if constexpr (UNIT) g = quad_unit_vjp<LPP>(g, ya, nrm_a);
     if (ok && scale != 0.f) scatter_quad<LPP>(dA, ba, sub, g);
     return;
   }
@@ -428,6 +563,7 @@ loss_lowres_bwd_quad_kernel(const float* __restrict__ la, const float* __restric
     const float oz = __shfl_down_sync(0xffffffffu, g.z, off * LPP), ow = __shfl_down_sync(0xffffffffu, g.w, off * LPP);
     if (take) { g.x += ox; g.y += oy; g.z += oz; g.w += ow; }
   }
+  if constexpr (UNIT) g = quad_unit_vjp<LPP>(g, ya, nrm_a);   // linear: the run's summed gradient takes the head's Jacobian once
   if (head && ok && (g.x != 0.f || g.y != 0.f || g.z != 0.f || g.w != 0.f)) scatter_quad<LPP>(dA, ba, sub, g);
 }
 
@@ -450,9 +586,21 @@ __global__ void add_f64_to_f32_kernel(const double* __restrict__ acc, float* __r
 
 using namespace ddn;
 
+static int check_lowres_flags(int flags) {
+  DDN_CHECK_ARG((flags & ~DDN_LOWRES_UNIT) == 0, "unknown low-resolution loss flags 0x%x", flags);
+  return 0;
+}
+
 extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
                                                     const ddn_loss_term* terms_host, int n_terms,
                                                     double* sums, int64_t* counts, void* stream) {
+  return ddn_contrastive_terms_forward_lowres_v2(low_a, low_b, B, h, w, H, W, D, terms_host, n_terms, sums, counts, 0, stream);
+}
+
+extern "C" int ddn_contrastive_terms_forward_lowres_v2(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
+                                                       const ddn_loss_term* terms_host, int n_terms,
+                                                       double* sums, int64_t* counts, int flags, void* stream) {
+  DDN_TRY(check_lowres_flags(flags));
   DDN_TRY(check_common(low_a, low_b, B, (int64_t)H * W, D, W));
   DDN_CHECK_ARG(sums && counts && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null outputs");
   const int lpp = (D == 8 || D == 16 || D == 32) ? D / 4 : 1;
@@ -468,8 +616,13 @@ extern "C" int ddn_contrastive_terms_forward_lowres(const float* low_a, const fl
   for (int i = 0; i < n_terms; ++i) pairs += (double)terms_host[i].n * B;
   ProfScope ps(PROF_LOSS_FWD, pairs * (16.0 + 8.0 * D), st);
   const float sh = ac_scale(h, H), sw = ac_scale(w, W);
-#define FWD(DT) DDN_LAUNCH(loss_lowres_fwd_kernel<DT>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, sums, cnt)
-#define FWDQ(L) DDN_LAUNCH(loss_lowres_fwd_quad_kernel<L>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt)
+  const bool unit = flags & DDN_LOWRES_UNIT;
+#define FWD(DT)                                                                                                                  \
+  if (unit) DDN_LAUNCH((loss_lowres_fwd_kernel<DT, true>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, sums, cnt); \
+  else DDN_LAUNCH((loss_lowres_fwd_kernel<DT, false>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, sums, cnt)
+#define FWDQ(L)                                                                                                                    \
+  if (unit) DDN_LAUNCH((loss_lowres_fwd_quad_kernel<L, true>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt); \
+  else DDN_LAUNCH((loss_lowres_fwd_quad_kernel<L, false>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, sums, cnt)
   switch (D) {
     case 3: FWD(3); break;
     case 4: FWD(4); break;
@@ -487,6 +640,15 @@ extern "C" int ddn_contrastive_terms_backward_lowres(const float* low_a, const f
                                                      const ddn_loss_term* terms_host, int n_terms,
                                                      const float* coef, const float* upstream,
                                                      float* dlow_a, float* dlow_b, double* scratch, void* stream) {
+  return ddn_contrastive_terms_backward_lowres_v2(low_a, low_b, B, h, w, H, W, D, terms_host, n_terms, coef, upstream, dlow_a, dlow_b,
+                                                  scratch, 0, stream);
+}
+
+extern "C" int ddn_contrastive_terms_backward_lowres_v2(const float* low_a, const float* low_b, int B, int h, int w, int H, int W, int D,
+                                                        const ddn_loss_term* terms_host, int n_terms,
+                                                        const float* coef, const float* upstream,
+                                                        float* dlow_a, float* dlow_b, double* scratch, int flags, void* stream) {
+  DDN_TRY(check_lowres_flags(flags));
   DDN_TRY(check_common(low_a, low_b, B, (int64_t)H * W, D, W));
   DDN_CHECK_ARG(coef && dlow_a && dlow_b && scratch && h >= 1 && w >= 1 && H >= h && W >= w && (int64_t)H * W < (1LL << 31), "bad low-resolution geometry / null buffers");
   DDN_CHECK_ARG(((reinterpret_cast<uintptr_t>(dlow_a) | reinterpret_cast<uintptr_t>(dlow_b) | reinterpret_cast<uintptr_t>(scratch) | reinterpret_cast<uintptr_t>(low_a) | reinterpret_cast<uintptr_t>(low_b)) & 15) == 0,
@@ -506,8 +668,13 @@ extern "C" int ddn_contrastive_terms_backward_lowres(const float* low_a, const f
   const float sh = ac_scale(h, H), sw = ac_scale(w, W);
   {
   ProfScope ps(PROF_LOSS_BWD, pairs * (16.0 + 24.0 * D), st);
-#define BWD(DT) DDN_LAUNCH(loss_lowres_bwd_kernel<DT>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, coef, upstream, dacc_a, dacc_b)
-#define BWDQ(L) DDN_LAUNCH(loss_lowres_bwd_quad_kernel<L>, grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, coef, upstream, dacc_a, dacc_b)
+  const bool unit = flags & DDN_LOWRES_UNIT;
+#define BWD(DT)                                                                                                                   \
+  if (unit) DDN_LAUNCH((loss_lowres_bwd_kernel<DT, true>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, coef, upstream, dacc_a, dacc_b); \
+  else DDN_LAUNCH((loss_lowres_bwd_kernel<DT, false>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, D, sh, sw, T, coef, upstream, dacc_a, dacc_b)
+#define BWDQ(L)                                                                                                                   \
+  if (unit) DDN_LAUNCH((loss_lowres_bwd_quad_kernel<L, true>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, coef, upstream, dacc_a, dacc_b); \
+  else DDN_LAUNCH((loss_lowres_bwd_quad_kernel<L, false>), grid, LR_THREADS, 0, st, low_a, low_b, h, w, H, W, sh, sw, T, coef, upstream, dacc_a, dacc_b)
   switch (D) {
     case 3: BWD(3); break;
     case 4: BWD(4); break;

@@ -110,28 +110,45 @@ class DenseCorrespondenceNetwork(nn.Module):
         res = self.fcn(img_tensor)
         if self._normalize:
             # net.py:256-259 -- as written upstream this only broadcasts for N == 1; kept, not fixed
+            tag = resnet_dilated.lowres_of(res)
             norm = torch.norm(res, 2, 1)
             res = res / norm
+            if tag is not None and res.shape[0] == 1:   # per pixel at N == 1: a fused loss normalises the blend the same way
+                resnet_dilated.attach_lowres(res, tag[0], tag[1], tag[2], unit=True)
         return res
 
-    def forward_pair(self, img_a, img_b):
+    def forward_pair(self, img_a, img_b, per_pixel_normalize=False):
         """(image_a_pred, image_b_pred) = (self.forward(img_a), self.forward(img_b)) -- the two forward calls of a reference
         training step (dense_correspondence/training/training.py:329-333) -- executed as ONE launch sequence over the
         concatenated batch with two BatchNorm groups: each image batch is normalised by its own batch statistics and the
         running statistics are updated A-then-B, exactly as the two calls would, but every kernel runs once on twice the
-        pixels (half the launches, better SM fill) and there is a single backward.  Opt-in: the reference API is two calls."""
+        pixels (half the launches, better SM fill) and there is a single backward.  Opt-in: the reference API is two calls.
+
+        ``per_pixel_normalize=True`` (only on a network built with ``normalize``): every pixel of every image is divided by
+        its own L2 norm, as each of the reference's batch-1 calls does (net.py:256-259), at any batch size.  Like
+        ``forward_pair`` itself this is the project's batched generalisation; the upsample kernel writes the unit descriptors
+        and the fused loss normalises its blended descriptors the same way.  A zero descriptor gives NaN, as in the
+        reference.  The default keeps the reference expression, which only broadcasts per pixel for a batch of one."""
         if img_a.shape != img_b.shape:
             raise ValueError("forward_pair needs two image batches of the same shape")
+        if per_pixel_normalize and not self._normalize:
+            raise ValueError("per_pixel_normalize=True needs a network built with normalize=True")
         B = img_a.shape[0]
-        res = self.fcn(torch.cat([img_a, img_b], 0), bn_groups=2)
+        if per_pixel_normalize:
+            res = self.fcn(torch.cat([img_a, img_b], 0), bn_groups=2, per_pixel_normalize=True)
+        else:
+            res = self.fcn(torch.cat([img_a, img_b], 0), bn_groups=2)
         res_a, res_b = res[:B], res[B:]
         tag = resnet_dilated.lowres_of(res)
         if tag is not None:
-            resnet_dilated.attach_lowres(res_a, tag[0][:B], tag[1], tag[2])
-            resnet_dilated.attach_lowres(res_b, tag[0][B:], tag[1], tag[2])
-        if self._normalize:
+            resnet_dilated.attach_lowres(res_a, tag[0][:B], tag[1], tag[2], unit=tag[4])
+            resnet_dilated.attach_lowres(res_b, tag[0][B:], tag[1], tag[2], unit=tag[4])
+        if self._normalize and not per_pixel_normalize:
             res_a = res_a / torch.norm(res_a, 2, 1)
             res_b = res_b / torch.norm(res_b, 2, 1)
+            if tag is not None and B == 1:      # per pixel at B == 1: a fused loss normalises the blend the same way
+                resnet_dilated.attach_lowres(res_a, tag[0][:B], tag[1], tag[2], unit=True)
+                resnet_dilated.attach_lowres(res_b, tag[0][B:], tag[1], tag[2], unit=True)
         return res_a, res_b
 
     def forward_single_image_tensor(self, img_tensor):
@@ -156,7 +173,7 @@ class DenseCorrespondenceNetwork(nn.Module):
         image_pred = image_pred.view(N, self.descriptor_dimension, W * H)
         image_pred = image_pred.permute(0, 2, 1)
         if tag is not None:       # a view of the same storage (shares the version counter): the tag stays valid
-            resnet_dilated.attach_lowres(image_pred, tag[0], tag[1], tag[2])
+            resnet_dilated.attach_lowres(image_pred, tag[0], tag[1], tag[2], unit=tag[4])
         return image_pred
 
     def clip_pixel_to_image_size_and_round(self, uv):

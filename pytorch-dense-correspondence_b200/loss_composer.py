@@ -20,15 +20,19 @@ from .resnet_dilated import lowres_of
 
 def _fused_lowres(image_a_pred, image_b_pred, image_width):
     """When both descriptor images are untouched outputs of Resnet34_8s (they carry the low-resolution map they were upsampled
-    from), the loss is evaluated THROUGH the upsample: (low_a, low_b, (h, w, H, W)), else None and the loss takes the generic
-    gather from the full-resolution images (a copy or any other tensor carries no such map)."""
+    from), the loss is evaluated THROUGH the upsample: (low_a, low_b, (h, w, H, W), unit), else None and the loss takes the
+    generic gather from the full-resolution images (a copy or any other tensor carries no such map).  ``unit``: both images
+    hold unit-length descriptors, so the fused loss normalises every blended descriptor; a pair whose images disagree on it
+    takes the generic gather."""
     ta, tb = lowres_of(image_a_pred), lowres_of(image_b_pred)
     if ta is None or tb is None or ta[1:3] != tb[1:3] or ta[2] != image_width or ta[0].shape != tb[0].shape:
+        return None
+    if ta[4] != tb[4]:
         return None
     H, W = ta[1], ta[2]
     if ta[0].dim() != 3 or ta[0].shape[1] != (H // 8) * (W // 8) or image_a_pred.shape[-2] != H * W:
         return None
-    return ta[0], tb[0], (H // 8, W // 8, H, W)
+    return ta[0], tb[0], (H // 8, W // 8, H, W), ta[4]
 
 
 class SpartanDatasetDataType:

@@ -46,15 +46,18 @@ def _check_precision(prec):
                            "(set DDN_TEST_FP32_SIMT=1 to use them); the product path is precision 'bf16x3' on the tensor cores")
 
 
-def attach_lowres(y, low, H, W):
+def attach_lowres(y, low, H, W, unit=False):
     """Tags a descriptor image with the low-resolution map it is the bilinear upsample of.  loss_composer looks for the tag and,
     when both images of a pair carry it, evaluates the loss through the 4 low-resolution cells of every sampled pixel
     (csrc/loss_lowres.cu) instead of gathering from the full-resolution tensor.  The tag records the tensor's version so that an
-    in-place modification of the image silently falls back to the generic path."""
-    y._ddn_lowres = (low, int(H), int(W), y._version)
+    in-place modification of the image silently falls back to the generic path.  ``unit=True``: the image is the upsample
+    with every pixel's descriptor normalised to unit length (the reference's ``normalize`` option, per pixel); the fused loss
+    then normalises each blended descriptor the same way.  -> tag ``(low, H, W, version, unit)``."""
+    y._ddn_lowres = (low, int(H), int(W), y._version, bool(unit))
 
 
 def lowres_of(t):
+    """The tag ``attach_lowres`` left on ``t``, or None when there is none or ``t`` was modified in place since."""
     tag = getattr(t, "_ddn_lowres", None)
     if tag is None or t._version != tag[3]:
         return None
@@ -80,7 +83,7 @@ class _Backbone(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, x, owner, groups, *params):
+    def forward(ctx, x, owner, groups, unit, *params):
         N.require_cuda_f32(x, "input image batch")
         if x.dim() != 4 or x.shape[1] != 3:
             raise RuntimeError("expected input of shape [N,3,H,W], got %s" % (tuple(x.shape),))
@@ -98,7 +101,8 @@ class _Backbone(torch.autograd.Function):
         _check_precision(prec)
         owner._register_weight_cache(flat, prec)
         arch = owner._ARCH
-        ws_bytes = N.lib.ddn_net_workspace_bytes(arch, B, H, W, D, mode, prec)
+        flags = N.NET_UNIT_DESCRIPTORS if unit else 0
+        ws_bytes = N.lib.ddn_net_workspace_bytes_v2(arch, B, H, W, D, mode, prec, flags)
         if ws_bytes == 0:
             raise N.DdnError("bad shape for %s: %s" % (type(owner).__name__, N.lib.ddn_last_error().decode()))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
@@ -106,13 +110,14 @@ class _Backbone(torch.autograd.Function):
         # the low-resolution map y is the bilinear upsample of, [B, H/8*W/8, D]: second output, so that a loss fused with the
         # upsample (contrastive_ops.within_scene_loss on tensors carrying `_ddn_lowres`) can differentiate through it directly
         low = torch.empty(B, (H // 8) * (W // 8), D, dtype=torch.float32, device=x.device)
-        N.check(N.lib.ddn_net_forward(arch, N.ptr(x), N.ptr(flat), N.ptr(bufs), N.ptr(y), N.ptr(ws), ws_bytes,
-                                      B, H, W, D, mode, groups, _BN_MOMENTUM, _BN_EPS, prec, N.ptr(low), N.stream_ptr()))
+        N.check(N.lib.ddn_net_forward_v2(arch, N.ptr(x), N.ptr(flat), N.ptr(bufs), N.ptr(y), N.ptr(ws), ws_bytes,
+                                         B, H, W, D, mode, groups, _BN_MOMENTUM, _BN_EPS, prec, N.ptr(low), flags, N.stream_ptr()))
         ctx.set_materialize_grads(False)
         if owner.training:
             torch._foreach_add_(owner._nbt, groups)
         if keep:
             ctx.owner, ctx.ws, ctx.shape, ctx.prec, ctx.mode, ctx.groups = owner, ws, (B, H, W, D), prec, mode, groups
+            ctx.flags = flags
             ctx.param_version = owner._flat_version
         ctx.keep = keep
         return y, low
@@ -120,7 +125,7 @@ class _Backbone(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy, dlow):
         if dy is None and dlow is None:
-            return (None, None, None) + (None,) * len(ctx.owner._params) if ctx.keep else None
+            return (None, None, None, None) + (None,) * len(ctx.owner._params) if ctx.keep else None
         if not ctx.keep:
             raise RuntimeError("backbone backward: nothing required a gradient in the forward; no activations were saved")
         if ctx.ws is None:
@@ -152,21 +157,22 @@ class _Backbone(torch.autograd.Function):
             def _on_bucket(_user, bucket, offset, numel, _g=grads, _h=hook):
                 _h.__call_bucket__(_g, int(bucket), int(offset), int(numel))
             cb = N.GRAD_BUCKET_FN(_on_bucket)
-        N.check(N.lib.ddn_net_backward(owner._ARCH, N.ptr(dy), N.ptr(dlow), N.ptr(flat), N.ptr(grads), N.ptr(ctx.ws), ctx.ws.numel(),
-                                       B, H, W, D, ctx.mode, ctx.groups, _BN_EPS, ctx.prec, cb, None, N.stream_ptr()))
+        N.check(N.lib.ddn_net_backward_v2(owner._ARCH, N.ptr(dy), N.ptr(dlow), N.ptr(flat), N.ptr(grads), N.ptr(ctx.ws),
+                                          ctx.ws.numel(), B, H, W, D, ctx.mode, ctx.groups, _BN_EPS, ctx.prec, ctx.flags, cb, None,
+                                          N.stream_ptr()))
         ctx.ws = None
         if hook is not None:
             hook.finish(grads)
         ps = owner._params
         if hook is None and owner._pad_index is not None:   # alignment padding between tensors: keep it zero (it is all-reduced / stepped too)
             grads.index_fill_(0, owner._pad_index_on(grads.device), 0.0)
-        wants = ctx.needs_input_grad[3:]
+        wants = ctx.needs_input_grad[4:]
         for p, want, (_, _, o, n) in zip(ps, wants, owner._ptab):
             if not want:
                 grads[o:o + n].zero_()      # frozen parameter: no gradient, and nothing for a flat optimizer / all-reduce to see
         if any(p._backward_hooks or getattr(p, "_post_accumulate_grad_hooks", None) for p in ps):
             # slow path: hand the per-tensor gradients to autograd (hooks, AccumulateGrad, autograd.grad all work)
-            return (None, None, None) + tuple(grads[o:o + n].view(s) if want else None
+            return (None, None, None, None) + tuple(grads[o:o + n].view(s) if want else None
                                               for want, (_, s, o, n) in zip(wants, owner._ptab))
         fg = owner._flat_grad
         fresh = fg is None or fg.device != grads.device
@@ -183,7 +189,7 @@ class _Backbone(torch.autograd.Function):
                     p.grad = grads[o:o + n].view(s)
         else:
             fg.add_(grads)
-        return (None, None, None) + (None,) * len(ps)
+        return (None, None, None, None) + (None,) * len(ps)
 
 
 class _DilatedResnet(nn.Module):
@@ -346,14 +352,18 @@ class _DilatedResnet(nn.Module):
         """The single fp32 array every parameter aliases (valid after the module is on its device)."""
         return self._ensure_flat(self._params[0].device)[0]
 
-    def forward(self, x, feature_alignment=False, bn_groups=1):
+    def forward(self, x, feature_alignment=False, bn_groups=1, per_pixel_normalize=False):
         """``bn_groups=2``: the batch is two consecutive groups (image-A batch, image-B batch), each normalised by its own
-        batch statistics -- the two forward calls of a reference training step in one launch sequence."""
+        batch statistics -- the two forward calls of a reference training step in one launch sequence.
+        ``per_pixel_normalize=True``: every pixel's descriptor is divided by its L2 norm inside the upsample kernel, image by
+        image (what the reference's ``normalize`` option computes for a batch of one); a zero descriptor gives NaN, as
+        ``x / ||x||`` does.  The output is tagged so that a fused loss normalises the same way."""
         if feature_alignment:
             raise NotImplementedError("feature_alignment=True is not on the dense-descriptor hot path "
                                       "(resnet_dilated.py:314 is never taken by the reference)")
-        y, low = _Backbone.apply(x, self, bn_groups, *self._params)
-        attach_lowres(y, low, x.shape[2], x.shape[3])
+        unit = bool(per_pixel_normalize)
+        y, low = _Backbone.apply(x, self, bn_groups, unit, *self._params)
+        attach_lowres(y, low, x.shape[2], x.shape[3], unit=unit)
         return y
 
 
