@@ -383,6 +383,27 @@ int ddn_conv2d_backward_data_bn_stats(const float* w_oihw, const float* dy_nhwc,
                                       int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int dil,
                                       int bn_groups, int precision, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The stem after conv1 (resnet.py:231-235: bn1 -> ReLU -> max-pool 3x3/2 pad 1), one operator at a time, with the kernels and the
+ * wiring the network runs.  raw [N,Hc,Wc,64] is conv1's output, mean / invstd [G][64] bn1's statistics per BatchNorm group
+ * (G = 1 or 2 dividing N: image n is in group n / (N/G)), gamma / beta [64]; Hp = (Hc-1)/2+1, Wp = (Wc-1)/2+1.
+ * Every argument is checked before anything is launched.
+ * Forward: y [N,Hp,Wp,64] = maxpool(relu(bn(raw))) as fp32 y and / or the bf16 planes y_hi = bf16(y), y_lo = bf16(y - y_hi)
+ * (y_lo may be NULL; the network writes it in BF16X3 only); argmax [N,Hp,Wp,64] uint8 = the window-local r*3+s of the first
+ * maximum in row-major scan order (a window whose every element is 0 after the ReLU: its first in-bounds element). */
+int ddn_stem_pool_forward(const float* raw, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                          float* y, void* y_hi_bf16, void* y_lo_bf16, void* argmax_u8, int N, int Hc, int Wc, int G, void* stream);
+/* Backward of the whole stem for the image x [N,3,H,W] (NCHW), Hc = (H-1)/2+1, Wc = (W-1)/2+1: dy_pool [N,Hp,Wp,64] -> the pool /
+ * ReLU backward g = scatter(dy_pool, argmax) * (bn(raw) > 0) -> bn1's backward (`training`: batch statistics; else frozen ones,
+ * dx = gamma * invstd * g) -> dgamma, dbeta [64] and dw_conv1 [64,3,7,7] (overwritten).  BF16X3 / BF16: the weight gradient
+ * runs on the tensor cores over the 7x7/2 patch planes of x and the bf16 planes of d raw; FP32_SIMT: the fp32 CUDA-core
+ * kernels over the NHWC4 image.  Optional outputs (NULL: not written): g_out and dx_bn [N,Hc,Wc,64] (the fp32 d raw), and on
+ * the tensor cores the bf16 planes of d raw the weight gradient reads, dx_hi = bf16(dx) and (BF16X3 only) dx_lo = bf16(dx - dx_hi). */
+size_t ddn_stem_workspace_bytes(int N, int H, int W, int precision);
+int ddn_stem_backward(const float* x_nchw, const float* raw, const float* mean, const float* invstd, const float* gamma,
+                      const float* beta, const void* argmax_u8, const float* dy_pool, float* g_out, float* dx_bn,
+                      void* dx_hi_bf16, void* dx_lo_bf16, float* dgamma, float* dbeta, float* dw_conv1,
+                      int N, int H, int W, int G, int training, int precision, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Bilinear align_corners=True resize of planar maps [N*C, h, w] -> [N*C, H, W]
  * (nn.functional.upsample_bilinear, resnet_dilated.py:320) and its adjoint. */
 int ddn_upsample_bilinear_forward(const float* x, float* y, int NC, int h, int w, int H, int W, void* stream);

@@ -155,6 +155,9 @@ _SIGNATURES = {
     "ddn_conv2d_bn_stats_forward": (i32, [vp] * 7 + [i32] * 10 + [f32, f32, i32, vp, sz, vp]),
     "ddn_conv2d_folded_forward": (i32, [vp] * 10 + [i32] * 10 + [f32, i32, vp, sz, vp]),
     "ddn_conv2d_backward_data_bn_stats": (i32, [vp] * 13 + [i32] * 11 + [vp, sz, vp]),
+    "ddn_stem_pool_forward": (i32, [vp] * 9 + [i32] * 4 + [vp]),
+    "ddn_stem_workspace_bytes": (sz, [i32] * 4),
+    "ddn_stem_backward": (i32, [vp] * 15 + [i32] * 6 + [vp, sz, vp]),
     "ddn_batchnorm_workspace_bytes": (sz, [i64, i32]),
     "ddn_batchnorm_forward": (i32, [vp] * 9 + [i64, i32, i32, i32, f32, f32, vp, sz, vp]),
     "ddn_batchnorm_backward": (i32, [vp] * 10 + [i64, i32, i32, vp, sz, vp]),

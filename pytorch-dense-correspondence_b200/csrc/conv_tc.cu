@@ -1200,15 +1200,6 @@ __global__ void stem_pack_weights_kernel(const float* __restrict__ w, __nv_bfloa
   if (want_lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
 }
 
-// dW'[co][192] -> conv1.weight gradient [64][3][7][7]
-__global__ void stem_unpack_wgrad_kernel(const float* __restrict__ dwk, float* __restrict__ dw) {
-  pdl_prologue();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 64 * 147) return;
-  int rs = i % 49, c = (i / 49) % 3, co = i / 147;
-  dw[i] = dwk[co * 192 + rs * 3 + c];
-}
-
 // ------------------------------------------------------------------------------------------------ weight-pack cache
 // The packed bf16 weights of every conv (forward and data-gradient layouts) live in a caller-owned cache that must never be
 // stale.  Staleness is decided ON THE DEVICE: every forward fingerprints the whole fp32 parameter array (two 64-bit sums
@@ -1708,15 +1699,10 @@ int tc_stem_forward(TcPlanes patches, const float* w_conv1, const TcPlanes* w_pa
   return tc_conv_planes(patches, nullptr, &wpk, raw, nullptr, stats, N, H1, W1, 192, 64, 1, 1, 1, 0, precision, wws, wws_bytes, st);
 }
 
-// d conv1.weight [64,3,7,7] from the patch planes and the planes of d(raw stem output).
-// dw_conv1 != nullptr: immediate (scratch: 64*192 doubles + 64*192 floats); else the pre-zeroed fp64 [64][192] accumulator
-// `scratch` is left for tc_unpack_wgrads.
-int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1, int W1, int precision, double* scratch, cudaStream_t st) {
-  if (!dw_conv1) return tc_wgrad_planes(patches, dy, nullptr, N, H1, W1, 192, 64, 1, 1, 1, precision, scratch, st);
-  double* dwp = scratch; float* dwk = reinterpret_cast<float*>(scratch + 64 * 192);
-  DDN_TRY(tc_wgrad_planes(patches, dy, dwk, N, H1, W1, 192, 64, 1, 1, 1, precision, dwp, st));
-  DDN_LAUNCH(stem_unpack_wgrad_kernel, (64 * 147 + 255) / 256, 256, 0, st, dwk, dw_conv1);
-  return 0;
+// d conv1.weight from the patch planes and the planes of d(raw stem output), accumulated into the pre-zeroed fp64 [64][192]
+// `dwp`, which tc_unpack_wgrads converts to [64][3][7][7] (a kind-1 entry).
+int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, int N, int H1, int W1, int precision, double* dwp, cudaStream_t st) {
+  return tc_wgrad_planes(patches, dy, nullptr, N, H1, W1, 192, 64, 1, 1, 1, precision, dwp, st);
 }
 
 // (re)packs every table entry into `cache` when the device-side fingerprint of params[0..n_params) differs from the one

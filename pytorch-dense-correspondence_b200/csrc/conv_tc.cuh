@@ -59,7 +59,7 @@ int tc_stem_patches(const float* x_nchw, __nv_bfloat16* hi, __nv_bfloat16* lo, i
 int tc_stem_pack_weights(const float* w_conv1, __nv_bfloat16* hi, __nv_bfloat16* lo, int precision, cudaStream_t st);   // [64][192]
 int tc_stem_forward(TcPlanes patches, const float* w_conv1, const TcPlanes* w_packed, float* raw, const BnFwdFinal* stats, int N, int H1,
                     int W1, int precision, void* wws, size_t wws_bytes, cudaStream_t st);
-int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, float* dw_conv1, int N, int H1, int W1, int precision, double* scratch, cudaStream_t st);
+int tc_stem_wgrad(TcPlanes patches, TcPlanes dy, int N, int H1, int W1, int precision, double* dwp, cudaStream_t st);   // [64][192] fp64
 
 // fp32-tensor wrappers (single-operator C ABI)
 // staging of those wrappers: weight packs, then the hi / lo planes of x, dy and the zero-inserted dy (x_el, dy_el, up_el elements)

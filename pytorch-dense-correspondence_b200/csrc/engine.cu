@@ -561,6 +561,20 @@ static int net_forward(const Ctx& c, const float* x, float* y, float* low_nhwc) 
   return 0;
 }
 
+// fp32 SIMT weight gradient of one conv: dw [Cout][Cin][k][k] (overwritten) through the zero-filled packed scratch `dwp`
+// [k*k*cin_eff*Cout] (cin_eff = Cin padded to the gather's channel count: 4 for the stem's NHWC4 image)
+static int simt_wgrad(const float* in, const float* dy, float* dwp, float* dw, int N, int Hin, int Win, int cin, int cin_eff, int Hout,
+                      int Wout, int cout, int k, int stride, int pad, int dil, cudaStream_t st) {
+  ConvGeom g;
+  DDN_TRY(conv_geom_init(&g, N, Hin, Win, cin_eff, Hout, Wout, cout, k, k, stride, 1, pad, dil));
+  DDN_TRY(launch_fill_zero(dwp, sizeof(float) * (size_t)k * k * cin_eff * cout, st));
+  {
+    ProfScope ps(PROF_CONV_WGRAD_SIMT, 2.0 * N * Hout * Wout * (double)cout * k * k * cin, st);
+    DDN_TRY(launch_conv_wgrad_f32(in, dy, dwp, g, st));
+  }
+  return launch_unpack_wgrad(dwp, dw, cout, cin, cin_eff, k, k, st);
+}
+
 // conv backward: dw -> grads (SIMT: immediately; tensor core: accumulated in dwp_all, converted per bucket), dx -> `dx`
 // (+ addend) when dx != nullptr.  Tensor-core convs take the saved bf16 planes of their input and the planes of dY
 // (p.grad_p, written by the BN backward that precedes this call); the fp32 SIMT convs take the fp32 tensors.
@@ -585,15 +599,7 @@ static int conv_backward(const Ctx& c, const ConvSpec& cs, const float* in, cons
     return 0;
   }
   DDN_CHECK_ARG(bst == nullptr, "backward statistics can only ride on a tensor-core data gradient");
-  ConvGeom g;
-  DDN_TRY(conv_geom_init(&g, N, Hin, Win, cin_eff, Hout, Wout, cs.cout, cs.k, cs.k, cs.stride, 1, cs.pad, cs.dil));
-  size_t wbytes = sizeof(float) * (size_t)cs.k * cs.k * cin_eff * cs.cout;
-  DDN_TRY(launch_fill_zero(c.f(p.dwp), wbytes, c.st));
-  {
-    ProfScope ps(PROF_CONV_WGRAD_SIMT, fl, c.st);
-    DDN_TRY(launch_conv_wgrad_f32(in, dy, c.f(p.dwp), g, c.st));
-  }
-  DDN_TRY(launch_unpack_wgrad(c.f(p.dwp), dw, cs.cout, cs.cin, cin_eff, cs.k, cs.k, c.st));
+  DDN_TRY(simt_wgrad(in, dy, c.f(p.dwp), dw, N, Hin, Win, cs.cin, cin_eff, Hout, Wout, cs.cout, cs.k, cs.stride, cs.pad, cs.dil, c.st));
   if (dx) {
     ConvGeom gd;
     DDN_TRY(conv_geom_init(&gd, N, Hout, Wout, cs.cout, Hin, Win, cs.cin, cs.k, cs.k, 1, cs.stride, cs.dil * (cs.k - 1) - cs.pad, cs.dil));
@@ -639,6 +645,44 @@ static bool bwd_stats_for(const Ctx& c, const BnSpec& bs, const ConvBufs& cb, co
   out->fin.a = c.accum(); out->fin.sums = c.sums(slot);
   out->fin.dgamma = c.grads + bs.g_off; out->fin.dbeta = c.grads + bs.b_off; out->fin.G = c.G; out->fin.C = bs.C;
   return true;
+}
+
+// The stem's backward: maxpool -> relu -> bn1 -> conv1 (weight gradient only; the image is not differentiated).  net_backward
+// runs it on its workspace, ddn_stem_backward on caller tensors.
+struct StemBwdArgs {
+  const float* dy_pool; const uint8_t* argmax;                       // [N,Hp,Wp,64]
+  const float* raw; const float* mean; const float* invstd;          // raw [N,H1,W1,64], statistics [G][64]
+  const float* gamma; const float* beta; float* dgamma; float* dbeta;
+  float* g;                       // [N,H1,W1,64]: the pre-BatchNorm gradient d(relu out) * (bn(raw) > 0)
+  float* dx;                      // [N,H1,W1,64]: d raw in fp32 -- the SIMT conv's dY; optional on the tensor cores
+  BnAccum acc; float* sums;       // BatchNorm-backward accumulator (zero) and [G][2][64] floats
+  // tensor cores: the 7x7/2 patch planes of the image, the planes of d raw, and the pre-zeroed fp64 [64][192] accumulator the
+  // caller converts (stem_unpack_entry)
+  TcPlanes patches; __nv_bfloat16* dx_hi; __nv_bfloat16* dx_lo; double* dwp;
+  // FP32_SIMT: the NHWC4 image, 7*7*4*64 floats of scratch, the conv1.weight gradient [64][3][7][7]
+  const float* x4; float* dwp_f32; float* dw;
+  int N, H, W, H1, W1, G, training, precision;
+};
+
+static int stem_backward(const StemBwdArgs& a, cudaStream_t st) {
+  DDN_TRY(launch_stem_pool_relu_backward(a.dy_pool, a.argmax, a.raw, a.mean, a.invstd, a.gamma, a.beta, a.g, a.N, a.H1, a.W1, 64, a.G, st));
+  const bool tc = a.precision != DDN_PRECISION_FP32_SIMT;
+  BnBwdArgs ks;
+  memset(&ks, 0, sizeof(ks));
+  ks.dy = a.g; ks.x = a.raw; ks.mean = a.mean; ks.invstd = a.invstd; ks.gamma = a.gamma; ks.beta = a.beta;
+  ks.dgamma = a.dgamma; ks.dbeta = a.dbeta; ks.acc = a.acc; ks.sums = a.sums;
+  ks.M = (int64_t)a.N * a.H1 * a.W1; ks.C = 64; ks.relu = 0; ks.training = a.training; ks.G = a.G;
+  ks.dx = a.dx;
+  if (tc) { ks.dx_hi = a.dx_hi; ks.dx_lo = a.precision == DDN_PRECISION_BF16X3 ? a.dx_lo : nullptr; }
+  DDN_TRY(launch_bn_backward(ks, st));
+  if (tc) return tc_stem_wgrad(a.patches, TcPlanes{a.dx_hi, a.dx_lo}, a.N, a.H1, a.W1, a.precision, a.dwp, st);
+  return simt_wgrad(a.x4, a.dx, a.dwp_f32, a.dw, a.N, a.H, a.W, 3, 4, a.H1, a.W1, 64, 7, 2, 3, 1, st);
+}
+
+// the conversion of the stem's [64][192] fp64 accumulator at dwp_base + src_off to conv1.weight at grads_base + dst_off
+static TcUnpackEntry stem_unpack_entry(int64_t src_off, int64_t dst_off) {
+  TcUnpackEntry e; e.src_off = src_off; e.dst_off = dst_off; e.Cout = 64; e.Cin = 3; e.taps = 49; e.kind = 1;
+  return e;
 }
 
 // gradient buckets, in the order the backward completes them (ddn_grad_bucket_fn): [first block of the layer .. next bucket)
@@ -736,29 +780,22 @@ static int net_backward(const Ctx& c, const float* dy, const float* dlow_nhwc, d
       if (i > 0) DDN_TRY(close_bucket(b.c[0].w_off));
     }
   }
-  // stem: maxpool -> relu -> bn1 -> conv1 (weight gradient only; the image is not differentiated)
-  int t1 = (cur + 1) & 3, t2 = (cur + 2) & 3;
-  DDN_TRY(launch_stem_pool_relu_backward(S[cur], reinterpret_cast<const uint8_t*>(c.ws + p.argmax), c.f(p.stem_raw),
-                                         c.mean(p.stem_stats), c.invstd(p.stem_stats, 64), c.params + s.stem_bn.g_off,
-                                         c.params + s.stem_bn.b_off, S[t1], B, p.H1, p.W1, 64, c.G, c.st));
-  BnBwdArgs ks;
-  memset(&ks, 0, sizeof(ks));
-  ks.dy = S[t1]; ks.x = c.f(p.stem_raw); ks.mean = c.mean(p.stem_stats); ks.invstd = c.invstd(p.stem_stats, 64);
-  ks.gamma = c.params + s.stem_bn.g_off; ks.beta = c.params + s.stem_bn.b_off;
-  ks.dgamma = c.grads + s.stem_bn.g_off; ks.dbeta = c.grads + s.stem_bn.b_off;
-  ks.acc = c.accum(); ks.sums = c.f(p.sums);
-  ks.M = (int64_t)B * p.H1 * p.W1; ks.C = 64; ks.relu = 0; ks.training = c.training() ? 1 : 0; ks.G = c.G;
+  // stem: maxpool -> relu -> bn1 -> conv1
+  StemBwdArgs sa;
+  memset(&sa, 0, sizeof(sa));
+  sa.dy_pool = S[cur]; sa.argmax = reinterpret_cast<const uint8_t*>(c.ws + p.argmax);
+  sa.raw = c.f(p.stem_raw); sa.mean = c.mean(p.stem_stats); sa.invstd = c.invstd(p.stem_stats, 64);
+  sa.gamma = c.params + s.stem_bn.g_off; sa.beta = c.params + s.stem_bn.b_off;
+  sa.dgamma = c.grads + s.stem_bn.g_off; sa.dbeta = c.grads + s.stem_bn.b_off;
+  sa.g = S[(cur + 1) & 3]; sa.acc = c.accum(); sa.sums = c.f(p.sums);
+  sa.N = B; sa.H = p.H; sa.W = p.W; sa.H1 = p.H1; sa.W1 = p.W1; sa.G = c.G; sa.training = c.training() ? 1 : 0; sa.precision = p.precision;
   if (p.tc) {
-    ks.dx_hi = c.h(p.grad_p.hi); ks.dx_lo = want_lo ? c.h(p.grad_p.lo) : nullptr;
-    DDN_TRY(launch_bn_backward(ks, c.st));
-    DDN_TRY(tc_stem_wgrad(c.planes(p.patch_p), c.planes(p.grad_p), nullptr, B, p.H1, p.W1, p.precision, c.d(p.dwp_all) + s.n_params, c.st));
-    TcUnpackEntry e; e.src_off = s.n_params; e.dst_off = s.stem.w_off; e.Cout = 64; e.Cin = 3; e.taps = 49; e.kind = 1;
-    pending.push_back(e);
+    sa.patches = c.planes(p.patch_p); sa.dx_hi = c.h(p.grad_p.hi); sa.dx_lo = c.h(p.grad_p.lo); sa.dwp = c.d(p.dwp_all) + s.n_params;
   } else {
-    ks.dx = S[t2];
-    DDN_TRY(launch_bn_backward(ks, c.st));
-    DDN_TRY(conv_backward(c, s.stem, c.f(p.x4), PlaneBufs{0, 0}, S[t2], nullptr, nullptr, B, p.H, p.W, p.H1, p.W1, 4));
+    sa.dx = S[(cur + 2) & 3]; sa.x4 = c.f(p.x4); sa.dwp_f32 = c.f(p.dwp); sa.dw = c.grads + s.stem.w_off;
   }
+  DDN_TRY(stem_backward(sa, c.st));
+  if (p.tc) pending.push_back(stem_unpack_entry(s.n_params, s.stem.w_off));
   return close_bucket(0);
 }
 
@@ -1159,4 +1196,86 @@ extern "C" int ddn_conv2d_backward_data_bn_stats(const float* w, const float* dy
   DDN_TRY(tc_split(dy, const_cast<__nv_bfloat16*>(pdy.hi), const_cast<__nv_bfloat16*>(pdy.lo), (int64_t)N * Ho * Wo * Cout, precision, st));
   return tc_conv_planes(pdy, w, nullptr, dx, addend, nullptr, N, H, W, Cin, Cout, k, 1, dil, 1, precision, wws, tc_weight_ws_bytes(), st,
                         nullptr, &bst);
+}
+
+// ---- the stem alone: the pool forward the network runs after conv1 + bn1 statistics, and the network's stem backward
+extern "C" int ddn_stem_pool_forward(const float* raw, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                                     float* y, void* y_hi, void* y_lo, void* argmax, int N, int Hc, int Wc, int G, void* stream) {
+  DDN_CHECK_ARG(raw && mean && invstd && gamma && beta && argmax, "null tensor");
+  DDN_CHECK_ARG(y || y_hi, "the pool needs an output: y and / or the y_hi plane");
+  DDN_CHECK_ARG(y_hi || !y_lo, "y_lo is the low plane of y_hi");
+  DDN_CHECK_ARG(N >= 1 && Hc >= 1 && Wc >= 1, "bad sizes N=%d Hc=%d Wc=%d", N, Hc, Wc);
+  DDN_TRY(check_groups(N, G));
+  return launch_stem_bn_relu_pool(raw, mean, invstd, gamma, beta, y, reinterpret_cast<uint8_t*>(argmax), (__nv_bfloat16*)y_hi,
+                                  (__nv_bfloat16*)y_lo, N, Hc, Wc, 64, G, (cudaStream_t)stream);
+}
+
+// workspace of ddn_stem_backward: byte offsets, 256-byte aligned
+struct StemWs { size_t acc, sums, g, dx, patch_hi, patch_lo, dx_hi, dx_lo, dwp, x4, dwp_f32, total; };
+static bool stem_ws_plan(int N, int H, int W, int precision, StemWs* w) {
+  if (N < 1 || H < 1 || W < 1 || precision < DDN_PRECISION_FP32_SIMT || precision > DDN_PRECISION_BF16) return false;
+  memset(w, 0, sizeof(*w));
+  size_t cur = 0;
+  auto alloc = [&](size_t bytes) { size_t o = cur; cur += align_up(bytes, 256); return o; };
+  const size_t m1 = (size_t)N * conv_out(H, 7, 2, 3, 1) * conv_out(W, 7, 2, 3, 1);
+  w->acc = alloc(bn_accum_bytes(64));
+  w->sums = alloc(sizeof(float) * 2 * BN_MAX_GROUPS * 64);
+  w->g = alloc(sizeof(float) * m1 * 64);
+  w->dx = alloc(sizeof(float) * m1 * 64);
+  if (precision != DDN_PRECISION_FP32_SIMT) {
+    w->patch_hi = alloc(2 * m1 * 192); w->patch_lo = alloc(2 * m1 * 192);
+    w->dx_hi = alloc(2 * m1 * 64); w->dx_lo = alloc(2 * m1 * 64);
+    w->dwp = alloc(sizeof(double) * 64 * 192);
+  } else {
+    w->x4 = alloc(sizeof(float) * (size_t)N * H * W * 4);
+    w->dwp_f32 = alloc(sizeof(float) * 7 * 7 * 4 * 64);
+  }
+  w->total = cur;
+  return true;
+}
+
+extern "C" size_t ddn_stem_workspace_bytes(int N, int H, int W, int precision) {
+  StemWs w;
+  return stem_ws_plan(N, H, W, precision, &w) ? w.total : 0;
+}
+
+extern "C" int ddn_stem_backward(const float* x_nchw, const float* raw, const float* mean, const float* invstd, const float* gamma,
+                                 const float* beta, const void* argmax, const float* dy_pool, float* g_out, float* dx_bn,
+                                 void* dx_hi, void* dx_lo, float* dgamma, float* dbeta, float* dw_conv1, int N, int H, int W, int G,
+                                 int training, int precision, void* workspace, size_t workspace_bytes, void* stream) {
+  DDN_CHECK_ARG(x_nchw && raw && mean && invstd && gamma && beta && argmax && dy_pool && dgamma && dbeta && dw_conv1, "null tensor");
+  DDN_CHECK_ARG(precision >= DDN_PRECISION_FP32_SIMT && precision <= DDN_PRECISION_BF16, "unknown precision %d", precision);
+  DDN_CHECK_ARG(N >= 1 && H >= 1 && W >= 1, "bad sizes N=%d H=%d W=%d", N, H, W);
+  DDN_TRY(check_groups(N, G));
+  const int H1 = conv_out(H, 7, 2, 3, 1), W1 = conv_out(W, 7, 2, 3, 1);
+  DDN_CHECK_ARG(N <= 65535 && H1 <= 65535, "stem: batch / height too large for the launch grid");
+  StemWs w;
+  stem_ws_plan(N, H, W, precision, &w);
+  DDN_CHECK_ARG(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be non-null and 256-byte aligned");
+  if (workspace_bytes < w.total) { set_error("workspace too small: %zu < %zu", workspace_bytes, w.total); return DDN_EWORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(ws + off); };
+  DDN_CUDA(cudaMemsetAsync(ws + w.acc, 0, bn_accum_bytes(64), st));
+  StemBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.dy_pool = dy_pool; a.argmax = reinterpret_cast<const uint8_t*>(argmax); a.raw = raw; a.mean = mean; a.invstd = invstd;
+  a.gamma = gamma; a.beta = beta; a.dgamma = dgamma; a.dbeta = dbeta;
+  a.g = g_out ? g_out : reinterpret_cast<float*>(ws + w.g);
+  a.acc = bn_accum_at(ws + w.acc, 64); a.sums = reinterpret_cast<float*>(ws + w.sums);
+  a.N = N; a.H = H; a.W = W; a.H1 = H1; a.W1 = W1; a.G = G; a.training = training ? 1 : 0; a.precision = precision;
+  if (precision == DDN_PRECISION_FP32_SIMT) {
+    a.x4 = reinterpret_cast<float*>(ws + w.x4); a.dwp_f32 = reinterpret_cast<float*>(ws + w.dwp_f32); a.dw = dw_conv1;
+    a.dx = dx_bn ? dx_bn : reinterpret_cast<float*>(ws + w.dx);
+    DDN_TRY(launch_nchw_to_nhwc4(x_nchw, const_cast<float*>(a.x4), N, H, W, st));
+    return stem_backward(a, st);
+  }
+  a.patches = TcPlanes{bf(w.patch_hi), bf(w.patch_lo)};
+  a.dx_hi = dx_hi ? (__nv_bfloat16*)dx_hi : bf(w.dx_hi); a.dx_lo = dx_lo ? (__nv_bfloat16*)dx_lo : bf(w.dx_lo);
+  a.dx = dx_bn; a.dwp = reinterpret_cast<double*>(ws + w.dwp);
+  DDN_CUDA(cudaMemsetAsync(a.dwp, 0, sizeof(double) * 64 * 192, st));
+  DDN_TRY(tc_stem_patches(x_nchw, bf(w.patch_hi), bf(w.patch_lo), N, H, W, precision, st));
+  DDN_TRY(stem_backward(a, st));
+  const TcUnpackEntry e = stem_unpack_entry(0, 0);
+  return tc_unpack_wgrads(&e, 1, a.dwp, dw_conv1, st);
 }

@@ -111,6 +111,45 @@ def conv2d_backward_data_bn_stats(w_oihw, dy, raw, mean, invstd, gamma, beta, st
     return dx, dgamma, dbeta, sums
 
 
+def stem_pool_forward(raw, mean, invstd, gamma, beta, want_y=True, want_planes=False, want_lo=True):
+    """The stem's bn1 -> ReLU -> max-pool 3x3/2 on conv1's output raw [N,Hc,Wc,64]; mean / invstd [G,64] per BatchNorm group.
+    -> (y [N,Hp,Wp,64] fp32 or None, y_hi bf16 or None, y_lo bf16 or None, argmax uint8 [N,Hp,Wp,64])"""
+    N.require_cuda_f32(raw, "raw")
+    n, hc, wc, c = raw.shape
+    assert c == 64
+    hp, wp = (hc - 1) // 2 + 1, (wc - 1) // 2 + 1
+    y = torch.empty(n, hp, wp, 64, dtype=torch.float32, device=raw.device) if want_y else None
+    y_hi = torch.empty(n, hp, wp, 64, dtype=torch.bfloat16, device=raw.device) if want_planes else None
+    y_lo = torch.empty_like(y_hi) if want_planes and want_lo else None
+    argmax = torch.empty(n, hp, wp, 64, dtype=torch.uint8, device=raw.device)
+    N.check(N.lib.ddn_stem_pool_forward(N.ptr(raw), N.ptr(mean), N.ptr(invstd), N.ptr(gamma), N.ptr(beta), N.ptr(y), N.ptr(y_hi),
+                                        N.ptr(y_lo), N.ptr(argmax), n, hc, wc, mean.shape[0], N.stream_ptr()))
+    return y, y_hi, y_lo, argmax
+
+
+def stem_backward(x, raw, mean, invstd, gamma, beta, argmax, dy_pool, training=True, want_g=False, want_dx=False,
+                  want_planes=False, precision=N.PRECISION_BF16X3):
+    """The network's stem backward (pool / ReLU -> bn1 -> conv1 weight gradient) for the NCHW image x [N,3,H,W].
+    want_planes (tensor cores): also the bf16 planes of d raw that the weight gradient reads (lo: BF16X3 only).
+    -> (dw_conv1 [64,3,7,7], dgamma [64], dbeta [64], g or None, dx_bn or None, dx_hi or None, dx_lo or None), [N,Hc,Wc,64] each"""
+    for t, name in ((x, "x"), (raw, "raw"), (dy_pool, "dy_pool")):
+        N.require_cuda_f32(t, name)
+    n, _, h, w = x.shape
+    dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=x.device)
+    dgamma = torch.empty(64, dtype=torch.float32, device=x.device)
+    dbeta = torch.empty_like(dgamma)
+    g = torch.empty_like(raw) if want_g else None
+    dx = torch.empty_like(raw) if want_dx else None
+    dx_hi = torch.empty(raw.shape, dtype=torch.bfloat16, device=x.device) if want_planes else None
+    dx_lo = torch.empty_like(dx_hi) if want_planes and precision == N.PRECISION_BF16X3 else None
+    ws = _ws(N.lib.ddn_stem_workspace_bytes(n, h, w, precision), x.device)
+    N.check(N.lib.ddn_stem_backward(N.ptr(x), N.ptr(raw), N.ptr(mean), N.ptr(invstd), N.ptr(gamma), N.ptr(beta), N.ptr(argmax),
+                                    N.ptr(dy_pool), N.ptr(g), N.ptr(dx), N.ptr(dx_hi), N.ptr(dx_lo), N.ptr(dgamma), N.ptr(dbeta),
+                                    N.ptr(dw), n, h, w, mean.shape[0], int(training), precision, N.ptr(ws), ws.numel(),
+                                    N.stream_ptr()))
+    return dw, dgamma, dbeta, g, dx, dx_hi, dx_lo
+
+
 def batchnorm_forward(x, gamma, beta, residual=None, relu=False, training=True, running_mean=None, running_var=None,
                       momentum=0.1, eps=1e-5):
     """x [..., C] channels-last.  -> (y, save_mean, save_invstd)"""

@@ -159,6 +159,52 @@ def test_fc_entries_refuse_before_any_launch():
     assert N.launch_count() == before
 
 
+def test_stem_entries_refuse_before_any_launch():
+    """ddn_stem_pool_forward / ddn_stem_backward check every argument before the first launch (fake, never dereferenced
+    pointers: each call below fails one check)."""
+    fake = ctypes.c_void_p(1 << 40)
+    X3, SIMT = N.PRECISION_BF16X3, N.PRECISION_FP32_SIMT
+    ws_x3 = N.lib.ddn_stem_workspace_bytes(2, 64, 96, X3)
+    ws_simt = N.lib.ddn_stem_workspace_bytes(2, 64, 96, SIMT)
+    m1 = 2 * 32 * 48
+    assert ws_x3 >= m1 * 64 * (4 + 4 + 2 + 2) + m1 * 192 * 4 + 64 * 192 * 8      # g, dx, dx planes, patch planes, fp64 dW
+    assert ws_simt >= m1 * 64 * 8 + 2 * 64 * 96 * 4 * 4                          # g, dx, the NHWC4 image
+    assert N.lib.ddn_stem_workspace_bytes(2, 64, 96, N.PRECISION_BF16) > 0
+    for n, h, w, prec in ((0, 64, 96, X3), (2, 0, 96, X3), (2, 64, 0, X3), (2, 64, 96, 3), (2, 64, 96, -1)):
+        assert N.lib.ddn_stem_workspace_bytes(n, h, w, prec) == 0
+
+    def pool(raw=fake, mean=fake, y=fake, y_hi=None, y_lo=None, argmax=fake, n=2, hc=32, wc=48, G=1):
+        return N.lib.ddn_stem_pool_forward(raw, mean, fake, fake, fake, y, y_hi, y_lo, argmax, n, hc, wc, G, None)
+
+    def bwd(x=fake, argmax=fake, dy=fake, dw=fake, dgamma=fake, n=2, h=64, w=96, G=1, prec=X3, ws=fake, nbytes=None):
+        nbytes = N.lib.ddn_stem_workspace_bytes(n, h, w, prec) if nbytes is None else nbytes
+        return N.lib.ddn_stem_backward(x, fake, fake, fake, fake, fake, argmax, dy, None, None, None, None, dgamma, fake, dw,
+                                       n, h, w, G, 1, prec, ws, nbytes, None)
+
+    before = N.launch_count()
+    assert pool(raw=None) == -1 and pool(mean=None) == -1 and pool(argmax=None) == -1     # null inputs / argmax
+    assert pool(y=None) == -1 and b"output" in N.lib.ddn_last_error()                      # no output at all
+    assert pool(y_lo=fake) == -1 and b"y_lo" in N.lib.ddn_last_error()                     # a lo plane without its hi plane
+    for kw in (dict(n=0), dict(hc=0), dict(wc=0)):
+        assert pool(**kw) == -1
+    for kw in (dict(G=3), dict(G=0), dict(n=3, G=2)):
+        assert pool(**kw) == -1 and b"bn_groups" in N.lib.ddn_last_error()
+    for kw in (dict(x=None), dict(argmax=None), dict(dy=None), dict(dw=None), dict(dgamma=None)):
+        assert bwd(**kw) == -1 and b"null" in N.lib.ddn_last_error()
+    for prec in (-1, 3):
+        assert bwd(prec=prec, nbytes=1 << 40) == -1 and b"precision" in N.lib.ddn_last_error()
+    for kw in (dict(n=0), dict(h=0), dict(w=0)):
+        assert bwd(nbytes=1 << 40, **kw) == -1 and b"sizes" in N.lib.ddn_last_error()
+    for kw in (dict(G=3), dict(G=0), dict(n=3, G=2)):
+        assert bwd(**kw) == -1 and b"bn_groups" in N.lib.ddn_last_error()
+    assert bwd(n=70000, G=1, nbytes=1 << 62) == -1 and b"launch grid" in N.lib.ddn_last_error()
+    for prec, nbytes in ((X3, ws_x3), (SIMT, ws_simt)):
+        assert bwd(prec=prec, nbytes=nbytes - 1) == -2 and b"workspace" in N.lib.ddn_last_error()
+    assert bwd(ws=None) == -1 and b"workspace" in N.lib.ddn_last_error()
+    assert bwd(ws=ctypes.c_void_p((1 << 40) + 128)) == -1 and b"256-byte" in N.lib.ddn_last_error()
+    assert N.launch_count() == before
+
+
 def test_batchnorm_workspace_covers_every_supported_width():
     """the standalone BatchNorm entries take the channel counts the kernels take, the network's 2048 included"""
     for C in (4, 64, 512, 1024, 2048, 4096):
