@@ -682,6 +682,18 @@ int ddn_synthetic_multi_object_batch(const ddn_smo_batch_cfg* cfg, const uint8_t
                                      const ddn_smo_batch_rand* rand, const ddn_smo_batch_out* out,
                                      void* scratch, size_t scratch_bytes, void* stream);
 
+/* Device-resident training frames (pdc_b200.frames.FrameStore): one launch gathers, for B pairs, frames idx_a[b] and
+ * idx_b[b] of a store of F frames of H x W -- rgb uint8 [F, H, W, 3], depth uint16 [F, H, W] (millimetres), mask uint8
+ * [F, H, W], contiguous -- into the producers' inputs: rgb_a / rgb_b uint8 [B, H, W, 3] and mask_a / mask_b uint8 [B, H, W]
+ * copied, depth_a / depth_b float32 [B, H, W] converted exactly (both null: no depth; across-scene pairs need none).
+ * The store may be in device memory or in pinned host memory (read through UVA, zero-copy); outputs are device memory.
+ * idx_a_host / idx_b_host are host arrays of B int32 in [0, F); they travel as kernel parameters, so the call neither copies
+ * nor synchronises.  B in [1, DDN_FRAMES_MAX_PAIRS]; every argument is checked before the launch. */
+#define DDN_FRAMES_MAX_PAIRS 128
+int ddn_frames_gather(const uint8_t* rgb, const uint16_t* depth, const uint8_t* mask, int64_t F, int H, int W,
+                      const int32_t* idx_a_host, const int32_t* idx_b_host, int B, uint8_t* rgb_a, uint8_t* rgb_b,
+                      float* depth_a, float* depth_b, uint8_t* mask_a, uint8_t* mask_b, void* stream);
+
 /* Fused Adam step over flat arrays == torch.optim.Adam(lr, betas, eps, weight_decay) as used by
  * dense_correspondence/training/training.py:133-145,346 (L2 weight decay folded into the gradient, bias-corrected moments,
  * no amsgrad).  `step` is the 1-based step count; grads are read as grads[i]*grad_scale (1/world after a SUM all-reduce). */

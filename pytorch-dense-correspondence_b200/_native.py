@@ -106,6 +106,7 @@ class SmoBatchOut(ctypes.Structure):
 
 
 SMO_MAX_PAIRS = WS_MAX_PAIRS // 2
+FRAMES_MAX_PAIRS = 128
 
 _SIGNATURES = {
     "ddn_abi_version": (i32, []),
@@ -182,6 +183,7 @@ _SIGNATURES = {
     "ddn_synthetic_multi_object_batch_scratch_bytes": (sz, [ctypes.POINTER(SmoBatchCfg)]),
     "ddn_synthetic_multi_object_batch": (i32, [ctypes.POINTER(SmoBatchCfg)] + [vp] * 9 + [ctypes.POINTER(SmoBatchRand),
                                                ctypes.POINTER(SmoBatchOut), vp, sz, vp]),
+    "ddn_frames_gather": (i32, [vp, vp, vp, i64, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]),
     "ddn_find_best_match": (i32, [vp, i64, i64, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ddn_match_statistics_scratch_bytes": (sz, [i32, i32, i32, i64]),
     "ddn_match_statistics": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,

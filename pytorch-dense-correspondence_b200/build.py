@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libddn_b200.so")
-SOURCES = ["engine.cu", "loss.cu", "loss_lowres.cu", "conv_simt.cu", "bn.cu", "head.cu", "conv_tc.cu", "optim.cu", "match.cu", "match_stats.cu", "descriptor_stats.cu", "sampling.cu", "within_scene.cu", "across_scene.cu", "synthetic_multi_object.cu"]
+SOURCES = ["engine.cu", "loss.cu", "loss_lowres.cu", "conv_simt.cu", "bn.cu", "head.cu", "conv_tc.cu", "optim.cu", "match.cu", "match_stats.cu", "descriptor_stats.cu", "sampling.cu", "within_scene.cu", "across_scene.cu", "synthetic_multi_object.cu", "frames.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "-cudart", "static"]

@@ -79,3 +79,50 @@ def plane_scene_pairs(B, H, W, seed, empty=()):
     dt = dict(rgb_a=torch.uint8, rgb_b=torch.uint8, depth_a=torch.float32, depth_b=torch.float32, mask_a=torch.uint8,
               mask_b=torch.uint8)
     return {k: torch.from_numpy(np.stack(v)).to(dt[k]) if k in dt else np.stack(v) for k, v in x.items()}, K
+
+
+def write_reference_scenes(root, scenes, H, W, seed=0, object_fraction=0.3):
+    """Write scenes in the reference's on-disk layout (SpartanDataset.get_image_filename / get_pose_data /
+    get_camera_intrinsics): ``root/<scene>/processed/images/%06d_rgb.png``, ``rendered_images/%06d_depth.png`` (16-bit
+    millimetres), ``image_masks/%06d_mask.png``, ``images/pose_data.yaml`` and ``images/camera_info.yaml``.
+    ``scenes``: {name: [(image index, quaternion (w, x, y, z), translation (x, y, z)), ...]}.  Each image is a ray-cast
+    tilted plane seen from its pose, with a smooth random RGB texture and a rectangular object mask covering about
+    ``object_fraction`` of it.  -> K, the 3x3 intrinsics written (scaled from 640x480)."""
+    import os
+    import yaml
+    from PIL import Image
+    from .frames import pose_from_dict
+    K = np.array([[533.6422696034836 * W / 640, 0, 319.4091030774892 * W / 640], [0, 534.7824445233571 * H / 480,
+                  236.4374299691866 * H / 480], [0, 0, 1.0]])
+    g = np.random.RandomState(seed)
+    us, vs = np.meshgrid(np.arange(W), np.arange(H))
+    rays = np.linalg.inv(K).dot(np.stack([us.ravel(), vs.ravel(), np.ones(H * W)]))
+    ramp = (np.stack([us / max(W - 1, 1), vs / max(H - 1, 1), (us + vs) / max(W + H - 2, 1)], axis=2) * 160).astype(np.int64)
+    side = np.sqrt(object_fraction)
+    for name, frames in scenes.items():
+        d = os.path.join(root, name, "processed")
+        for sub in ("images", "rendered_images", "image_masks"):
+            os.makedirs(os.path.join(d, sub), exist_ok=True)
+        pose_data = {}
+        for idx, q, t in frames:
+            cam = {"quaternion": dict(zip("wxyz", map(float, q))), "translation": dict(zip("xyz", map(float, t)))}
+            pose_data[int(idx)] = {"camera_to_world": cam, "rgb_image_filename": "%06d_rgb.png" % idx,
+                                   "depth_image_filename": "%06d_depth.png" % idx}
+            T4 = pose_from_dict(cam)
+            nrm, d0 = np.array([-0.1, 0.05, 1.0]), 1.2 + float(T4[2, 3])
+            s = (d0 - nrm.dot(T4[:3, 3])) / nrm.dot(T4[:3, :3].dot(rays))
+            depth = np.clip(np.round(s * 1000.0), 0, 65535).reshape(H, W).astype(np.uint16)
+            rgb = np.clip(ramp + g.randint(0, 64, (1, 1, 3)) + g.randint(0, 32, (H, W, 3)), 0, 255).astype(np.uint8)
+            mask = np.zeros((H, W), dtype=np.uint8)
+            h, w = max(1, int(H * side)), max(1, int(W * side))
+            y0, x0 = g.randint(0, H - h + 1), g.randint(0, W - w + 1)
+            mask[y0:y0 + h, x0:x0 + w] = 1
+            Image.fromarray(rgb).save(os.path.join(d, "images", "%06d_rgb.png" % idx))
+            Image.fromarray(depth).save(os.path.join(d, "rendered_images", "%06d_depth.png" % idx))
+            Image.fromarray(mask).save(os.path.join(d, "image_masks", "%06d_mask.png" % idx))
+        with open(os.path.join(d, "images", "pose_data.yaml"), "w") as f:
+            yaml.safe_dump(pose_data, f, default_flow_style=False)
+        with open(os.path.join(d, "images", "camera_info.yaml"), "w") as f:
+            yaml.safe_dump({"camera_matrix": {"cols": 3, "rows": 3, "data": [float(v) for v in K.ravel()]},
+                            "image_width": W, "image_height": H}, f, default_flow_style=False)
+    return K
